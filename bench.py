@@ -24,6 +24,11 @@ CUDA events around its launches (gsicp_prof_*); `cpu_baseline` = the reference's
 /root/reference into oracle/_ref) + the CPU raster oracle on a bounded sample.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c3|c2|c4|c5] [--multi replicas|shard]
+                  [--dump-outputs DIR]
+`--dump-outputs DIR` writes what the headline run's last timed step returned to its caller (pose, correspondences, loss,
+rendered images, radii, parameter gradients) as DIR/<name>.npy in float32 / float64, at most 60 MB (per-Gaussian arrays
+are cut to a fixed, seeded sample of Gaussians beyond that), for comparing two builds output for output: the inputs
+depend on the arguments only.
 `--impl reference` = the reference's own implementation of the same frame on this box: fast_gicp (its unmodified
 sources + pybind module, oracle/_ref/fast_gicp) on all host cores in a tracker process + the reference's CUDA
 rasterizer through its own torch extension (oracle/_ref/site, stock build path) and PyTorch loss in the mapper process.
@@ -66,6 +71,8 @@ def parse():
                          "c1: GICP align of two 10k-point clouds (the reference's CPU-runnable case); "
                          "c4 / c5: the large rasterizer-only / GICP-only strong-scaling configs")
     ap.add_argument("--gaussians", type=int, default=None)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of the headline run as DIR/<name>.npy (c3 / c2, --impl ours)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
     ap.add_argument("--no-variants", action="store_true", help="skip the fused-loss and back-to-back passes")
@@ -259,6 +266,8 @@ class Ours:
         self.pool = None
         self.gicp_stream = None
         self.stats = dict(R=0, V=0, n_src=0, n_corr=0, n_tgt=0, frames=0, h2d=0, d2h=0, n_lin=0, pose_err=0.0)
+        self.keep_outputs = False  # hold on to each step's results for --dump-outputs (references only, no copies)
+        self.last_outputs = {}
         self.refresh_target(resident=True)
 
     def set_loss(self, kind):
@@ -296,6 +305,8 @@ class Ours:
         st["n_lin"] += self.reg.last_iterations
         st["pose_err"] = max(st["pose_err"], float(np.abs(pose.astype(np.float64) - f["c2w"]).max()))
         self.pose = pose
+        if self.keep_outputs:
+            self.last_outputs.update(pose=pose, correspondences=corr, squared_distances=sqd)
         if (step + 1) % KEYFRAME_EVERY == 0:
             rots, scales = self.reg.get_source_rotationsq(), self.reg.get_source_scales()
             st["d2h"] += rots.nbytes + scales.nbytes
@@ -332,6 +343,9 @@ class Ours:
         loss.backward()
         lv = float(loss.item())  # D2H read of the step's result
         st["d2h"] += 8
+        if self.keep_outputs:
+            self.last_outputs.update(loss=lv, color=color, depth=depth, radii=radii, grad_means2D=self.means2D.grad,
+                                     **{"grad_" + k: v.grad for k, v in m.items()})
         for k in m:
             m[k].grad = None
         self.means2D.grad = None
@@ -596,7 +610,7 @@ def reference_arm(args):
     t_trk, pose_err = msg[1], msg[2]
     proc.join(timeout=10)
     fps = args.steps / dt
-    mapper = ("reference CUDA rasterizer through its own torch extension (oracle/_ref/site, sm_100a) + PyTorch loss on cuda:0"
+    mapper = ("reference CUDA rasterizer through its own torch extension (oracle/_ref/site, sm_90a) + PyTorch loss on cuda:0"
               if use_gpu else "CPU raster oracle (1 thread)")
     tracker = ("fast_gicp (reference sources + pybind module, oracle/_ref/fast_gicp; PCL k-NN through oracle/pcl_shim)"
                if kind == "reference" else "oracle restatement of fast_gicp")
@@ -632,12 +646,40 @@ def workload_config(args, label, **extra):
 
 
 def ncu_traffic():
-    """DRAM bytes per launch from the committed ncu capture of this build (profiles/ncu_traffic.json, written by
-    tools/ncu_summary.py); None when no capture has been summarised."""
+    """DRAM bytes and warp instructions per launch from an ncu capture of this build, summarised into
+    profiles/ncu_traffic.json by tools/ncu_summary.py; {} (roofline.traffic null, no roofline.issue) until one is taken."""
     try:
         return json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
     except Exception:
         return {}
+
+
+DUMP_LIMIT = 60_000_000  # bytes of array data written by --dump-outputs (the .npy headers add 128 bytes a file)
+
+
+def dump_outputs(out_dir, outputs, n_gaussians):
+    """DIR/<name>.npy for every output of a step: float32 arrays and integers below 2**24 as float32, other integers and the
+    loss as float64.  When the whole set would pass DUMP_LIMIT, the per-Gaussian arrays (radii, grad_*) keep a fixed, seeded
+    sample of Gaussians, whose indices are written as gaussian_rows.npy."""
+    import torch
+
+    arrays = {}
+    for name, v in outputs.items():
+        a = v.detach().cpu().numpy() if torch.is_tensor(v) else np.asarray(v)
+        small_int = a.dtype.kind in "iu" and (a.size == 0 or int(np.abs(a).max()) < (1 << 24))
+        arrays[name] = a.astype(np.float32) if (a.dtype.kind == "f" and a.dtype.itemsize <= 4) or small_int else a.astype(np.float64)
+    per_gaussian = [k for k in arrays if k == "radii" or k.startswith("grad_")]
+    if sum(a.nbytes for a in arrays.values()) > DUMP_LIMIT:
+        other = sum(a.nbytes for k, a in arrays.items() if k not in per_gaussian)
+        per_row = 8 + sum(arrays[k].nbytes // n_gaussians for k in per_gaussian)
+        keep = max(0, min(n_gaussians, (DUMP_LIMIT - other) // per_row))
+        rows = np.sort(np.random.default_rng(0).choice(n_gaussians, size=keep, replace=False))
+        for k in per_gaussian:
+            arrays[k] = arrays[k][rows]
+        arrays["gaussian_rows"] = rows.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def bind_to_gpu_numa(local_rank, world):
@@ -675,6 +717,10 @@ def main():
     rank = int(os.environ.get("RANK", 0))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
+    if args.dump_outputs is not None and (args.config in ("c1", "c4", "c5") or args.impl != "ours"
+                                          or (world > 1 and args.multi == "shard")):
+        raise SystemExit("bench.py: --dump-outputs covers the SLAM frame of --impl ours (--config c3 or c2, not --multi shard, "
+                         "whose ranks each hold a part of the frame)")
     if args.config in ("c1", "c4", "c5"):
         from tools import bench_large
 
@@ -727,8 +773,12 @@ def main():
         eng.enable_concurrent(concurrent)
         if concurrent:
             eng.run(pre, 1, resident=True)  # stream / thread start-up, untimed
+        eng.keep_outputs = args.dump_outputs is not None
         r = eng.run(K, Wm, resident=True)
+        eng.keep_outputs = False
         res_times = list(eng.last_times)
+        if args.dump_outputs is not None and rank == 0:
+            dump_outputs(args.dump_outputs, eng.last_outputs, args.gaussians)
         e = eng.run(K, Wm, resident=False)
         e2e_times = list(eng.last_times)
     clocks = clk.summary()
@@ -774,7 +824,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json)") if "hbm_gbs" in peaks else (6650.0, "fallback (B200_PROFILING.md)")
+    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json)") if "hbm_gbs" in peaks else (3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)")
 
     roofline, kernels = None, {}
     if prof:
@@ -813,10 +863,11 @@ def main():
                     "ms_per_launch": kernels[top]["ms_per_launch"]}
         if tr.get("warp_instructions"):
             a = tr["warp_instructions"] / (kernels[top]["ms_per_launch"] * 1e-3) / 1e9
-            pk = 148 * 4 * ((clocks or {}).get("sm_mhz") or 1965.0) * 1e6 / 1e9
+            pk = 132 * 4 * ((clocks or {}).get("sm_mhz") or 1980.0) * 1e6 / 1e9
             roofline["issue"] = {"warp_instructions_per_launch": tr["warp_instructions"], "achieved": a, "peak": pk,
                                  "unit": "G warp-inst/s", "frac": a / pk,
-                                 "note": "instruction count from the committed ncu capture; peak = 148 SMs x 4 schedulers x SM clock"}
+                                 "note": "instruction count from an ncu capture summarised into profiles/ncu_traffic.json by tools/ncu_summary.py; "
+                                         "peak = 132 SMs x 4 schedulers x SM clock (H100 SXM)"}
         if "render_forward" in kernels and "render_backward" in kernels:
             roofline["render_fwd_bwd_GBps"] = ((alg["render_forward"] + alg["render_backward"]) / 1e9 /
                                               ((kernels["render_forward"]["ms_per_launch"] + kernels["render_backward"]["ms_per_launch"]) * 1e-3))

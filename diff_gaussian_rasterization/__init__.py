@@ -1,4 +1,4 @@
-"""Drop-in `diff_gaussian_rasterization` backed by libgsicp_b200.so (sm_100a).
+"""Drop-in `diff_gaussian_rasterization` backed by libgsicp_b200.so (sm_90a).
 
 Public surface = the reference package's
 (submodules/diff-gaussian-rasterization/diff_gaussian_rasterization/__init__.py:44-222):

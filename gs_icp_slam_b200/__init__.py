@@ -1,4 +1,4 @@
-"""gs_icp_slam_b200 — B200-native (sm_100a) hot paths of GS-ICP-SLAM behind the reference's APIs.
+"""gs_icp_slam_b200 — H100-native (sm_90a) hot paths of GS-ICP-SLAM behind the reference's APIs.
 
   rasterizer  : Gaussian-splat rasterizer forward/backward  (diff_gaussian_rasterization drop-in)
   gicp        : Generalized-ICP tracker                      (pygicp drop-in)

@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libgsicp_b200.so")
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
-        f"{LIB_PATH} is missing: build the sm_100a CUDA library first "
+        f"{LIB_PATH} is missing: build the sm_90a CUDA library first "
         "(make -C gs_icp_slam_b200/csrc). gs_icp_slam_b200 has no CPU fallback."
     )
 

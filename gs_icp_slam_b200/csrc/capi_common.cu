@@ -107,7 +107,7 @@ extern "C" const char* gsicp_last_error(void) { return gsicp::g_err; }
 #define GSICP_STR2(x) #x
 #define GSICP_STR(x) GSICP_STR2(x)
 extern "C" const char* gsicp_build_info(void) {
-  return "libgsicp_b200 sm_100a (CUDA " GSICP_STR(CUDART_VERSION) ", built " __DATE__ ")";
+  return "libgsicp_b200 sm_90a (CUDA " GSICP_STR(CUDART_VERSION) ", built " __DATE__ ")";
 }
 
 extern "C" uint64_t gsicp_launch_count(void) { return gsicp::g_launches.load(); }

@@ -47,6 +47,14 @@ struct ProfScope {
   ~ProfScope() { if (g_prof_on) prof_end(k, s); }
 };
 
+// Multiprocessors of the current device: persistent and grid-stride kernels size their grids by it.
+inline int device_sm_count() {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return 1;  // the launch that follows reports the device error
+  return sms > 0 ? sms : 1;
+}
+
 // Grow-only device scratch buffer (library-internal workspace that backward does not need).
 struct Scratch {
   void* ptr = nullptr;

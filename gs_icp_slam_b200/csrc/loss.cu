@@ -14,6 +14,7 @@
 // convolution with the same window gives d(mean ssim)/dx without ever materialising the 121-tap adjoint.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 
 #include "host_common.h"
@@ -26,7 +27,10 @@ constexpr int kHalo = kWin / 2;
 constexpr int kLossIn = kLossTile + 2 * kHalo;  // 26
 constexpr int kLossThreads = 128;                // 104 threads work in the horizontal pass, 64 in the vertical one
 constexpr int kLossCtasPerSm = 10;
-constexpr int kLossFwdCtas = 148 * kLossCtasPerSm;  // forward grid: persistent CTAs walking (tile, channel) items
+// forward grid: kLossCtasPerSm persistent CTAs per SM walking (tile, channel) items; the partial-sum slots of the work
+// buffer are sized for up to kLossMaxSms multiprocessors so that its size does not depend on the device
+constexpr int kLossMaxSms = 256;
+constexpr int kLossFwdCtas = kLossMaxSms * kLossCtasPerSm;
 
 struct LossWindow {
   float w[kWin];
@@ -411,7 +415,8 @@ int gsicp_mapping_loss_forward(int H, int W, const float* d_image, const float* 
   }
   cudaStream_t stream = (cudaStream_t)stream_;
   const int items = ((W + kLossTile - 1) / kLossTile) * ((H + kLossTile - 1) / kLossTile) * 4;
-  const int grid = items < kLossFwdCtas ? items : kLossFwdCtas;
+  const int ctas = std::min(device_sm_count(), kLossMaxSms) * kLossCtasPerSm;
+  const int grid = items < ctas ? items : ctas;
   LossArgs a;
   a.H = H; a.W = W; a.image = d_image; a.depth = d_depth; a.gt_image = d_gt_image; a.gt_depth = d_gt_depth;
   a.lambda_dssim = lambda_dssim; a.depth_weight = depth_weight; a.inv_dmax = 1.f / d_max;

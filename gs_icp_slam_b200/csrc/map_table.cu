@@ -205,7 +205,7 @@ extern "C" int gsicp_adam_step(int n_tensors, float* const* d_params, const floa
     t.step_size[j] = (float)((double)lrs[k] / bc1);
   }
   if (total == 0) return GSICP_OK;
-  const int blocks = (int)std::min<unsigned long long>((total + 255) / 256, 148ull * 16);
+  const int blocks = (int)std::min<unsigned long long>((total + 255) / 256, 16ull * device_sm_count());  // 16 CTAs per SM
   GSICP_LAUNCH(adam_kernel, blocks, 256, 0, (cudaStream_t)stream_v, t, total, (float)(1.0 - beta1), (float)beta2,
                (float)(1.0 - beta2), (float)(1.0 / bc2_sqrt), (float)eps);
   GSICP_CUDA(cudaGetLastError());

@@ -1,4 +1,4 @@
-// raster_backward.cu — backward pass of the B200 Gaussian-splat rasterizer.
+// raster_backward.cu — backward pass of the H100 Gaussian-splat rasterizer.
 //
 // Replaces CudaRasterizer::Rasterizer::backward (DGR/cuda_rasterizer/rasterizer_impl.cu:351-454):
 //   BACKWARD::render (backward.cu:429-657)  +  computeCov2DCUDA (:144-294)  +  preprocessCUDA (:369-426)

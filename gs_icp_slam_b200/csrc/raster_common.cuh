@@ -1,4 +1,4 @@
-// raster_common.cuh — shared types and per-Gaussian math of the B200 Gaussian-splat rasterizer.
+// raster_common.cuh — shared types and per-Gaussian math of the H100 Gaussian-splat rasterizer.
 //
 // Data layout in HBM (DESIGN.md §3): every visible Gaussian is reduced by `preprocess` to ONE
 // 48-byte "splat record" (3 x float4, 16-B aligned) that both render kernels read with three

@@ -1,4 +1,4 @@
-// raster_forward.cu — forward pass of the B200 Gaussian-splat rasterizer.
+// raster_forward.cu — forward pass of the H100 Gaussian-splat rasterizer.
 //
 // Replaces CudaRasterizer::Rasterizer::forward (DGR/cuda_rasterizer/rasterizer_impl.cu:201-347):
 //   preprocess -> scan -> duplicateWithKeys -> 64-bit radix sort of all R instances -> identifyTileRanges -> render

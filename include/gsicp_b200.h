@@ -1,5 +1,5 @@
 /*
- * gsicp_b200.h — C ABI of libgsicp_b200.so (sm_100a).
+ * gsicp_b200.h — C ABI of libgsicp_b200.so (sm_90a).
  *
  * Drop-in boundary for the two data-parallel hot paths of GS-ICP-SLAM
  * (SURVEY.md §8b).  Every entry point cites the reference interface it
@@ -32,7 +32,7 @@ extern "C" {
 #define GSICP_ESTATE (-4)   /* call sequence error (e.g. align() without target) */
 
 const char* gsicp_last_error(void);
-/* "sm_100a" + build flags; lets host code verify the native library is the one loaded. */
+/* "sm_90a" + build flags; lets host code verify the native library is the one loaded. */
 const char* gsicp_build_info(void);
 /* Number of kernel launches issued by this library since process start (bench.py: gpu_launches). */
 uint64_t gsicp_launch_count(void);

@@ -1,7 +1,7 @@
 #!/bin/bash
 # oracle/build_ref_ext.sh — TEST INFRASTRUCTURE.  Installs the reference's OWN PyTorch extensions, unmodified and
 # through their own setup.py (torch.utils.cpp_extension, i.e. the stock build path: rasterize_points.cu + ext.cpp,
-# torch caching allocator, current-stream semantics as upstream), for sm_100a into oracle/_ref/site/:
+# torch caching allocator, current-stream semantics as upstream), for sm_90a into oracle/_ref/site/:
 #     diff_gaussian_rasterization (+ _C)   from $REF/submodules/diff-gaussian-rasterization
 #     simple_knn (+ _C)                    from $REF/submodules/simple-knn   (needs <cfloat>: NVCC_APPEND_FLAGS)
 # The source trees are read-only, so pip builds from a scratch copy under /tmp.  Nothing is copied into the repo:
@@ -23,7 +23,7 @@ trap 'rm -rf "$TMP"' EXIT
 cp -r "$REF/submodules/diff-gaussian-rasterization" "$TMP/dgr"
 cp -r "$REF/submodules/simple-knn" "$TMP/sk"
 mkdir -p "$OUT"
-export TORCH_CUDA_ARCH_LIST="10.0a" MAX_JOBS=${MAX_JOBS:-8} FORCE_CUDA=1
+export TORCH_CUDA_ARCH_LIST="9.0a" MAX_JOBS=${MAX_JOBS:-8} FORCE_CUDA=1
 python -m pip install --no-index --no-build-isolation --no-deps --upgrade --target "$OUT" "$TMP/dgr"
 NVCC_APPEND_FLAGS="-include cfloat" python -m pip install --no-index --no-build-isolation --no-deps --upgrade --target "$OUT" "$TMP/sk"
 ls -la "$OUT" "$OUT/diff_gaussian_rasterization" "$OUT/simple_knn"

@@ -1,6 +1,6 @@
 """ctypes binding of oracle/_ref/libref_cuda.so — the REFERENCE's own CUDA rasterizer / simple-knn compiled
-unmodified for sm_100a (oracle/Makefile, oracle/ref_shim.cu).  GPU only.  Test infrastructure and the
-"reference kernels on the same B200" timing leg of bench.py."""
+unmodified for sm_90a (oracle/Makefile, oracle/ref_shim.cu).  GPU only.  Test infrastructure (golden generation) and
+the "reference kernels on the same GPU" timing leg of the tools."""
 import ctypes as C
 import os
 

@@ -3,7 +3,7 @@
 //   submodules/diff-gaussian-rasterization/cuda_rasterizer/{forward,backward,rasterizer_impl}.cu
 //   submodules/simple-knn/simple_knn.cu
 // into oracle/_ref/libref_cuda.so.  TEST INFRASTRUCTURE: used by tests/ (GPU parity, golden-vector
-// generation) and by bench.py's per-kernel "reference CUDA on the same B200" comparison only.
+// generation) and by bench.py's per-kernel "reference CUDA on the same GPU" comparison only.
 //
 // Everything below is our own glue: it calls the reference's public C++ interface
 // (cuda_rasterizer/rasterizer.h:22-88, simple_knn.h:15-19) with device pointers supplied by the caller.

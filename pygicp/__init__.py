@@ -1,4 +1,4 @@
-"""Drop-in `pygicp` module backed by libgsicp_b200.so (sm_100a CUDA), for the reference's
+"""Drop-in `pygicp` module backed by libgsicp_b200.so (sm_90a CUDA), for the reference's
 mp_Tracker.py / mp_Tracker_unlimit.py (`self.reg = pygicp.FastGICP()`, mp_Tracker.py:53).
 
 Exports the class the trackers use.  The other registrations the reference binds (FastVGICP,

@@ -1,6 +1,7 @@
 """Call sequences shared by the GICP parity tests.  Every case takes a `make()` factory returning an object with the
-pygicp.FastGICP interface (this repo's CUDA drop-in, the CPU oracle, or the reference's own pybind11 module built from
-/root/reference: oracle/ref_gicp.py) and returns a dict of numpy results to compare."""
+pygicp.FastGICP interface (this repo's CUDA drop-in, the CPU oracle, or the reference's own pybind11 module built by
+`make -C oracle ref`: oracle/ref_gicp.py) and returns a dict of numpy results to compare, with each other (compare) or with
+the golden record of the reference's run (compare_golden)."""
 import os
 
 import numpy as np
@@ -99,6 +100,26 @@ def compare(a, b, exact_prefixes=("corr", "sqd", "tgt_rots", "src_rots", "tgt_sc
             assert np.abs(x - y).max() <= h_rtol * np.abs(y).max(), (k, np.abs(x - y).max() / np.abs(y).max())
         elif k.startswith(exact_prefixes):
             assert np.array_equal(x, y), (k, int((x != y).sum()), x.size)
+        else:
+            raise AssertionError(f"unclassified key {k}")
+
+
+def compare_golden(a, rec, pose_tol=1e-6, h_rtol=1e-9, exact_prefixes=compare.__defaults__[0]):
+    """compare(a, reference run) with the reference's run given as its golden record (tests/refgold.py)."""
+    for k in a:
+        if k in ("T_gt", "relative", "gt_last"):
+            continue
+        assert k in rec, f"{k} missing from the golden record"
+        if k.startswith("pose"):
+            x, y = np.asarray(a[k]), rec.full(k)
+            assert x.shape == y.shape and x.dtype == y.dtype, (k, x.dtype, y.dtype)
+            assert np.abs(x.astype(np.float64) - y.astype(np.float64)).max() <= pose_tol, k
+        elif k.startswith("H"):
+            x, y = np.asarray(a[k]), rec.full(k)
+            assert x.shape == y.shape and x.dtype == y.dtype, (k, x.dtype, y.dtype)
+            assert np.abs(x - y).max() <= h_rtol * np.abs(y).max(), (k, np.abs(x - y).max() / np.abs(y).max())
+        elif k.startswith(exact_prefixes):
+            rec.exact(k, a[k])
         else:
             raise AssertionError(f"unclassified key {k}")
 

@@ -1,6 +1,6 @@
 """Generates tests/golden/raster_ref_small.npz from the REFERENCE's own CUDA rasterizer (oracle/_ref/libref_cuda.so,
-built unmodified from /root/reference for sm_100a).  Needs a GPU:
-    gpurun -- 'python tests/golden/make_raster_golden.py && cp tests/golden/raster_ref_small.npz gpurun_out/'
+built unmodified from the reference's sources by `make -C oracle ref`).  Needs a GPU:
+    python tests/golden/make_raster_golden.py
 The fixture pins oracle/raster_oracle.c (tests/test_raster_oracle.py, CPU) and the CUDA path (tests/test_raster_gpu.py)
 to outputs of the reference itself: colour, depth, radii, is_used, num_rendered, sorted point_list, ranges, 8 gradients."""
 import os

@@ -27,15 +27,15 @@ def test_library_exports_every_declared_symbol():
     missing = [s for s in declared if s not in exported]
     assert not missing, f"declared in include/gsicp_b200.h but not exported: {missing}"
     assert set(declared) <= set(_lib.BOUND) | {"gsicp_test_set_render_cull", "gsicp_test_set_bwd_variant"}
-    assert b"sm_100a" in _lib.lib.gsicp_build_info()
+    assert b"sm_90a" in _lib.lib.gsicp_build_info()
 
 
-def test_library_contains_sm100a_code_only():
+def test_library_contains_sm90a_code_only():
     from gs_icp_slam_b200 import _lib
 
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_dropin_modules_import_and_expose_reference_surface():

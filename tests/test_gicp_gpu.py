@@ -223,6 +223,12 @@ def test_edge_cases(cuda):
     assert isinstance(r2, pygicp.FastGICP) and r2.get_source_rotationsq().size == 0
 
 
+def dist2_big_cloud(cuda):
+    import torch
+
+    return torch.from_numpy(S.sample_surface(200000, 41, 0.002)[0].astype(np.float32)).to(cuda)
+
+
 def test_dist2_matches_bruteforce_and_reference(cuda):
     import torch
     from simple_knn._C import distCUDA2
@@ -234,12 +240,15 @@ def test_dist2_matches_bruteforce_and_reference(cuda):
     np.fill_diagonal(d, np.inf)
     ref = np.sort(d, axis=1)[:, :3].mean(1)
     assert np.allclose(out, ref, rtol=2e-5, atol=1e-12)
-    from oracle import ref_cuda
+    # the reference's simple-knn on 200k points (golden record: tests/golden/make_raster_ref_cases_golden.py)
+    from tests.refgold import Record
 
-    if ref_cuda.available():
-        big = torch.from_numpy(S.sample_surface(200000, 41, 0.002)[0].astype(np.float32)).to(cuda)
-        a, b = distCUDA2(big), ref_cuda.ref_dist2(big)
-        assert torch.allclose(a, b, rtol=2e-5, atol=1e-12)
+    rec = Record(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "raster_ref_cases.npz"), "dist2_200k")
+    a = distCUDA2(dist2_big_cloud(cuda)).cpu().numpy()
+    if not rec.same("dist2", a):
+        assert rec.finite_matches("dist2", a)
+        _, x, y, _ = rec.sample("dist2", a)
+        assert np.allclose(x, y, rtol=2e-5, atol=1e-12)
     assert torch.isinf(distCUDA2(torch.zeros((2, 3), device=cuda))).all()  # fewer than 3 neighbours -> inf, like FLT_MAX sums
 
 

@@ -1,5 +1,6 @@
 """CPU tests: the GICP oracle (oracle/gicp_oracle.cpp) against
-  * the reference's vendored Eigen (oracle/_ref/libref_gicp_eigen.so: JacobiSVD, Quaterniond, inverse, LDLT),
+  * the reference's vendored Eigen (JacobiSVD, Quaterniond, inverse, LDLT through oracle/gicp_eigen_ref.cpp), replayed
+    from the calls recorded in tests/golden/eigen_ref_calls.npz (tests/golden/make_reference_cpu_golden.py),
   * brute-force numpy k-NN,
   * the committed golden vectors (tests/golden/gicp_*.npz), incl. the reference's own acceptance fixture
     (KITTI pair + relative.txt, bound 0.05 m / 1 deg: submodules/fast_gicp/src/test/gicp_test.cpp:147-201)."""
@@ -13,14 +14,13 @@ from gs_icp_slam_b200 import synthetic as S
 from oracle import gicp_oracle as G
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-EIG = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "libref_gicp_eigen.so")
 
 
-@pytest.fixture(scope="module")
-def eig():
-    if not os.path.exists(EIG):
-        pytest.skip("oracle/_ref/libref_gicp_eigen.so not built (needs /root/reference)")
-    return C.CDLL(EIG)
+@pytest.fixture()
+def eig(request):
+    from tests import refgold
+
+    return refgold.EigenReplay(os.path.join(HERE, "golden", "eigen_ref_calls.npz"), request.node.originalname)
 
 
 def _p(a):
@@ -167,7 +167,7 @@ def test_linearize_matches_eigen_per_point(eig):
     Pf = pose.astype(np.float32)
     s32, t32 = src.astype(np.float32), tgt.astype(np.float32)
     # (c0 x + c1 y) + (c2 z + c3): the order Eigen's packet product evaluates trans_f * getVector4fMap() (fgi:260), pinned
-    # against the reference build in tests/test_gicp_reference.py
+    # against the reference's fast_gicp in tests/test_gicp_reference.py
     tp = (Pf[:3, 0] * s32[:, [0]] + Pf[:3, 1] * s32[:, [1]]) + (Pf[:3, 2] * s32[:, [2]] + Pf[:3, 3])
     d = (tp[:, None, :] - t32[None, :, :]).astype(np.float32) ** 2
     d2 = (d[..., 0] + d[..., 1]) + d[..., 2]

@@ -1,4 +1,4 @@
-"""Multi-GPU parity (needs >= 2 GPUs; run with `gpurun --gpus 2 -- python -m pytest tests/test_multigpu_gpu.py -m gpu`):
+"""Multi-GPU parity (needs >= 2 GPUs; skipped on a single-GPU machine; run with `python -m pytest tests/test_multigpu_gpu.py -m gpu`):
 tile-sharded rasterizer + point-sharded GICP must reproduce the single-GPU results, through both transports: the
 library's in-kernel exchange over peer memory (CUDA IPC / NVLink) and the NCCL-callback fallback."""
 import os

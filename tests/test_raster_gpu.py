@@ -1,14 +1,53 @@
 """GPU parity of the rasterizer: our CUDA path (through the C ABI) vs
-  (1) the reference's own CUDA code compiled unmodified for sm_100a (oracle/_ref/libref_cuda.so), and
+  (1) the reference's own CUDA code (its rasterizer through oracle/ref_shim.cu, and its own torch extension), compiled
+      unmodified for sm_90a and run on an H100 on the same inputs; its outputs are golden records in
+      tests/golden/raster_ref_*.npz (tests/golden/make_raster_ref_cases_golden.py; tests/refgold.py), and
   (2) the CPU restatement oracle/raster_oracle.c.
 Tolerances (BASELINE.json north_star): indices bit-exact; rendered L1 <= 1e-4, PSNR within 0.01 dB."""
+import os
+
 import numpy as np
 import pytest
 import torch
 
+from tests.refgold import Record
 from tests.util import psnr, rel_err, scene_tensors
 
 pytestmark = pytest.mark.gpu
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+GRADS = ["means2D", "colors", "opacity", "means3D", "cov3D", "sh", "scales", "rotations"]
+EXT_GRADS = ["means3D", "shs", "opacities", "scales", "rotations", "means2D"]
+
+
+def gold_file(case):
+    """The golden file of a case: the torch-extension and full-size cases have files of their own (1 MB per file)."""
+    kind = case.split("_")[0]
+    return os.path.join(GOLDEN, f"raster_ref_{kind}.npz" if kind in ("ext", "full") else "raster_ref_cases.npz")
+
+
+def _gold(case):
+    return Record(gold_file(case), case)
+
+
+def _np(x):
+    return x.cpu().numpy() if torch.is_tensor(x) else np.asarray(x)
+
+
+def _pix(img):
+    """(C, H, W) image -> (H*W, C) array: the layout images are recorded in, so that sampled rows are pixels."""
+    img = _np(img)
+    return np.ascontiguousarray(img.reshape(img.shape[0], -1).T)
+
+
+def _exact_forward(g, n, radii, is_used, pl, rg, color=None, depth=None):
+    """Instance count, radii, visibility, sorted instance list and tile ranges (and the images) bit-identical."""
+    assert n == int(g.full("num_rendered"))
+    for name, x in (("radii", radii), ("is_used", is_used), ("point_list", pl), ("ranges", rg)):
+        if x is not None:
+            g.exact(name, _np(x))
+    for name, x in (("color", color), ("depth", depth)):
+        if x is not None:
+            g.exact(name, _pix(x))
 
 
 def _ours(t, c, H, W, bg, degree=0, colors=None, cov=None):
@@ -22,111 +61,48 @@ def _ours(t, c, H, W, bg, degree=0, colors=None, cov=None):
 
 
 def _ref(t, c, H, W, bg, degree=0):
+    """The reference rasterizer on the same inputs (golden generation only)."""
     from oracle import ref_cuda
 
-    if not ref_cuda.available():
-        pytest.skip("oracle/_ref/libref_cuda.so not built")
     return ref_cuda.RefRaster(bg, t["means3D"], t["shs"], None, t["opacities"].reshape(-1), t["scales"], t["rotations"],
                               None, c["viewmatrix"], c["projmatrix"], c["campos"], c["tanfovx"], c["tanfovy"], H, W, degree)
 
 
-@pytest.mark.parametrize("P,size,degree,seed", [(20000, (320, 240), 0, 2), (100000, (640, 480), 0, 3), (30000, (333, 211), 3, 5)])
-def test_forward_backward_vs_reference_cuda(cuda, P, size, degree, seed):
-    from gs_icp_slam_b200 import rasterizer as R
+def ref_outputs(ref, gcol=None, gdep=None):
+    """What the tests compare of a reference run (golden generation only)."""
+    pl, rg = ref.export()
+    out = dict(num_rendered=np.array(ref.num_rendered, np.int64), radii=ref.radii, is_used=ref.is_used, point_list=pl,
+               ranges=rg, color=_pix(ref.color), depth=_pix(ref.depth))
+    if gcol is not None:
+        g = ref.backward(gcol, gdep)
+        out.update({"grad_" + k: g[k] for k in GRADS})
+    ref.free()
+    return {k: _np(v) for k, v in out.items()}
 
+
+# ---- inputs of each case, shared by the tests and tests/golden/make_raster_ref_cases_golden.py ----
+def case_fb(cuda, P, size, degree, seed):
     g, cm, t, c, cam = scene_tensors(P, seed, cuda, sh_degree=degree, size=size)
-    W, H = size
-    bg = torch.tensor([0.1, 0.2, 0.3], device=cuda)
-    n, depth, color, radii, is_used, geom, binning, img = _ours(t, c, H, W, bg, degree)
-    ref = _ref(t, c, H, W, bg, degree)
-
-    # ---- indexing: bit-exact ----
-    assert n == ref.num_rendered
-    assert torch.equal(radii, ref.radii)
-    assert torch.equal(is_used, ref.is_used)
-    pl, rg = R.export_binning(n, H, W, binning, img)
-    rpl, rrg = ref.export()
-    assert torch.equal(rg, rrg)
-    assert torch.equal(pl, rpl)
-
-    # ---- image: L1 / PSNR ----
-    col, rcol = color.cpu().numpy(), ref.color.cpu().numpy()
-    dep, rdep = depth.cpu().numpy(), ref.depth.cpu().numpy()
-    assert np.abs(col - rcol).mean() <= 1e-4
-    assert np.abs(col - rcol).max() <= 2e-3
-    assert np.abs(dep - rdep).mean() <= 1e-4
-    assert psnr(col, rcol) >= 80.0  # i.e. PSNR against any target differs by << 0.01 dB
-
-    # ---- gradients ----
     gen = torch.Generator(device="cpu").manual_seed(seed + 5)
+    W, H = size
     gcol = torch.randn((3, H, W), generator=gen).to(cuda)
     gdep = torch.randn((1, H, W), generator=gen).to(cuda)
-    e = torch.Tensor([])
-    ours = R.rasterize_gaussians_backward(bg, t["means3D"], radii, e, t["scales"], t["rotations"], 1.0, e, c["viewmatrix"],
-                                          c["projmatrix"], c["tanfovx"], c["tanfovy"], gdep, gcol, t["shs"], degree,
-                                          c["campos"], geom, n, binning, img, False)
-    names = ["means2D", "colors", "opacity", "means3D", "cov3D", "sh", "scales", "rotations"]
-    rgrad = ref.backward(gcol, gdep)
-    for name, o in zip(names, ours):
-        r = rgrad[name]
-        if name == "colors":
-            continue  # the reference returns dL_dcolors only as an internal when SHs are used; compare below
-        err = rel_err(o.cpu().numpy(), r.cpu().numpy())
-        assert err <= 2e-4, f"grad {name}: rel err {err}"
-    assert rel_err(ours[1].cpu().numpy(), rgrad["colors"].cpu().numpy()) <= 2e-4
-    ref.free()
+    return t, c, torch.tensor([0.1, 0.2, 0.3], device=cuda), gcol, gdep
 
 
-@pytest.mark.parametrize("active_degree,scale_modifier,size", [(2, 0.7, (250, 190)), (1, 1.6, (96, 64)), (0, 1.0, (17, 33))])
-def test_options_vs_reference_cuda(cuda, active_degree, scale_modifier, size):
-    """SH table larger than the active degree (the SLAM raises active_sh_degree over time), scale_modifier != 1, image
-    sizes that are not multiples of the 16x16 tile, non-zero background."""
-    from gs_icp_slam_b200 import rasterizer as R
-    from oracle import ref_cuda
-
-    if not ref_cuda.available():
-        pytest.skip("oracle/_ref/libref_cuda.so not built")
+def case_options(cuda, active_degree, size):
     g, cm, t, c, cam = scene_tensors(15000, 40 + active_degree, cuda, sh_degree=3, size=size)
     W, H = size
-    bg = torch.tensor([0.7, 0.1, 0.4], device=cuda)
-    e = torch.Tensor([])
-    n, depth, color, radii, is_used, geom, binning, img = R.rasterize_gaussians(
-        bg, t["means3D"], e, t["opacities"], t["scales"], t["rotations"], scale_modifier, e, c["viewmatrix"], c["projmatrix"],
-        c["tanfovx"], c["tanfovy"], H, W, t["shs"], active_degree, c["campos"], False, False)
-    ref = ref_cuda.RefRaster(bg, t["means3D"], t["shs"], None, t["opacities"].reshape(-1), t["scales"], t["rotations"], None,
-                             c["viewmatrix"], c["projmatrix"], c["campos"], c["tanfovx"], c["tanfovy"], H, W, active_degree,
-                             scale_modifier=scale_modifier)
-    assert n == ref.num_rendered and n > 0
-    assert torch.equal(radii, ref.radii) and torch.equal(is_used, ref.is_used)
-    pl, rg = R.export_binning(n, H, W, binning, img)
-    rpl, rrg = ref.export()
-    assert torch.equal(rg, rrg) and torch.equal(pl, rpl)
-    assert torch.equal(color, ref.color) and torch.equal(depth, ref.depth)  # bit-identical images
     gen = torch.Generator(device="cpu").manual_seed(77)
     gcol = torch.randn((3, H, W), generator=gen).to(cuda)
     gdep = torch.randn((1, H, W), generator=gen).to(cuda)
-    ours = R.rasterize_gaussians_backward(bg, t["means3D"], radii, e, t["scales"], t["rotations"], scale_modifier, e,
-                                          c["viewmatrix"], c["projmatrix"], c["tanfovx"], c["tanfovy"], gdep, gcol, t["shs"],
-                                          active_degree, c["campos"], geom, n, binning, img, False)
-    rgrad = ref.backward(gcol, gdep)
-    for name, o in zip(["means2D", "colors", "opacity", "means3D", "cov3D", "sh", "scales", "rotations"], ours):
-        assert rel_err(o.cpu().numpy(), rgrad[name].cpu().numpy()) <= 2e-4, name
-    # SH coefficients above the active degree receive no gradient
-    assert float(ours[5][:, (active_degree + 1) ** 2:, :].abs().max()) == 0.0
-    # mark_visible (rasterize_points.cu:208-227) = the near-plane test of the forward pass
-    vis = R.mark_visible(t["means3D"], c["viewmatrix"], c["projmatrix"])
-    assert bool((vis | (radii == 0)).all())
-    ref.free()
+    return t, c, torch.tensor([0.7, 0.1, 0.4], device=cuda), gcol, gdep
 
 
-def test_degenerate_gaussians_vs_reference_cuda(cuda):
-    """Finite but extreme inputs: zero scales (only the 0.3 px low-pass is left), 1 km scales (the rectangle is the whole
-    screen), saturated and vanishing opacities, Gaussians exactly on the near plane and on the camera centre."""
+def case_degenerate(cuda):
+    """Finite but extreme inputs; returns the 40 modified Gaussians' indices too."""
     from gs_icp_slam_b200 import rasterizer as R
-    from oracle import ref_cuda
 
-    if not ref_cuda.available():
-        pytest.skip("oracle/_ref/libref_cuda.so not built")
     g, cm, t, c, cam = scene_tensors(3000, 17, cuda, size=(200, 152))
     W, H = 200, 152
     with torch.no_grad():
@@ -142,36 +118,165 @@ def test_degenerate_gaussians_vs_reference_cuda(cuda):
         t["means3D"][a[33]] = c["campos"] + 0.2000001 * fwd
         t["means3D"][a[34]] = c["campos"]                        # the camera centre
         t["rotations"][a[35]] = 0.0                              # zero quaternion (the reference does not normalise)
-    bg = torch.tensor([0.3, 0.6, 0.9], device=cuda)
-    n, depth, color, radii, is_used, geom, binning, img = _ours(t, c, H, W, bg)
-    ref = _ref(t, c, H, W, bg)
-    assert n == ref.num_rendered and torch.equal(radii, ref.radii) and torch.equal(is_used, ref.is_used)
-    pl, rg = R.export_binning(n, H, W, binning, img)
-    rpl, rrg = ref.export()
-    assert torch.equal(rg, rrg) and torch.equal(pl, rpl)
-    assert torch.equal(color.view(torch.int32), ref.color.view(torch.int32))   # bit patterns (robust to inf / nan)
-    assert torch.equal(depth.view(torch.int32), ref.depth.view(torch.int32))
     gen = torch.Generator(device="cpu").manual_seed(3)
     gcol = torch.randn((3, H, W), generator=gen).to(cuda)
     gdep = torch.randn((1, H, W), generator=gen).to(cuda)
+    return t, c, torch.tensor([0.3, 0.6, 0.9], device=cuda), gcol, gdep, a
+
+
+def case_precomputed(cuda):
+    P, (W, H) = 30000, (320, 240)
+    g, cm, t, c, cam = scene_tensors(P, 23, cuda, size=(W, H))
+    gen = torch.Generator(device="cpu").manual_seed(1)
+    colors = torch.rand((P, 3), generator=gen).to(cuda)
+    # Sigma = Rm diag(s^2) Rm^T with Rm the rotation of the (x,y,z,w) quaternion (forward.cu:122-168), upper triangle
+    q, s = t["rotations"].double(), t["scales"].double()
+    x, y, z, w = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
+    Rm = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y), 2 * (x * y + w * z),
+                      1 - 2 * (x * x + z * z), 2 * (y * z - w * x), 2 * (x * z - w * y), 2 * (y * z + w * x),
+                      1 - 2 * (x * x + y * y)], 1).view(P, 3, 3)
+    Sg = Rm @ torch.diag_embed(s * s) @ Rm.transpose(1, 2)
+    cov = torch.stack([Sg[:, 0, 0], Sg[:, 0, 1], Sg[:, 0, 2], Sg[:, 1, 1], Sg[:, 1, 2], Sg[:, 2, 2]], 1).float().contiguous()
+    gcol = torch.randn((3, H, W), generator=gen).to(cuda)
+    gdep = torch.randn((1, H, W), generator=gen).to(cuda)
+    return t, c, torch.tensor([0.2, 0.1, 0.4], device=cuda), colors, cov, gcol, gdep
+
+
+def case_crowded(cuda, P):
+    g, cm, t, c, cam = scene_tensors(P, 31, cuda, size=(160, 120))
+    # pull every Gaussian towards a point 2 m in front of the camera so that a few tiles hold thousands of instances
+    centre = c["campos"] + 2.0 * c["viewmatrix"][:3, 2]  # viewmatrix = (world->view)^T: column 2 is the optical axis
+    t["means3D"] = (centre + 0.02 * (t["means3D"] - t["means3D"].mean(0))).contiguous()
+    t["means3D"][100:200] = t["means3D"][300:400]  # exact duplicates: equal depth keys, order decided by the index
+    return t, c, torch.zeros(3, device=cuda)
+
+
+def case_ext(cuda, P, size, degree, seed):
+    g, cm, t, c, cam = scene_tensors(P, seed, cuda, sh_degree=degree, size=size)
+    W, H = size
+    gen = torch.Generator(device="cpu").manual_seed(11)
+    gcol = torch.randn((3, H, W), generator=gen).to(cuda)
+    gdep = torch.randn((1, H, W), generator=gen).to(cuda)
+    active = max(degree - 1, 0) if degree == 3 else degree  # degree-3 table rendered at degree 2: the tail gets zero grads
+    return t, c, torch.tensor([0.1, 0.2, 0.3], device=cuda), gcol, gdep, active
+
+
+def run_ext(mod, t, c, H, W, bg, gcol, gdep, active):
+    """One forward + two backward passes (the second on the retained graph) through a diff_gaussian_rasterization module."""
+    p = {k: v.detach().clone().requires_grad_(True) for k, v in t.items()}
+    m2 = torch.zeros_like(p["means3D"], requires_grad=True)
+    rs = mod.GaussianRasterizationSettings(H, W, c["tanfovx"], c["tanfovy"], bg, 1.0, c["viewmatrix"], c["projmatrix"],
+                                           active, c["campos"], False, False)
+    depth, color, radii, is_used = mod.GaussianRasterizer(rs)(means3D=p["means3D"], means2D=m2, opacities=p["opacities"],
+                                                              shs=p["shs"], scales=p["scales"], rotations=p["rotations"])
+    loss = (color * gcol).sum() + (depth * gdep).sum()
+    loss.backward(retain_graph=True)
+    g1 = {k: v.grad.clone() for k, v in p.items()}
+    g1["means2D"] = m2.grad.clone()
+    for v in p.values():
+        v.grad = None
+    m2.grad = None
+    loss.backward()  # second backward on the same saved state
+    g2 = {k: v.grad.clone() for k, v in p.items()}
+    g2["means2D"] = m2.grad.clone()
+    return depth.detach(), color.detach(), radii, is_used, g1, g2
+
+
+FB_CASES = [(20000, (320, 240), 0, 2), (100000, (640, 480), 0, 3), (30000, (333, 211), 3, 5)]
+
+
+@pytest.mark.parametrize("P,size,degree,seed", FB_CASES)
+def test_forward_backward_vs_reference_cuda(cuda, P, size, degree, seed):
+    from gs_icp_slam_b200 import rasterizer as R
+
+    t, c, bg, gcol, gdep = case_fb(cuda, P, size, degree, seed)
+    W, H = size
+    n, depth, color, radii, is_used, geom, binning, img = _ours(t, c, H, W, bg, degree)
+    ref = _gold(f"fb_{P}_{degree}_{seed}")
+
+    # ---- indexing: bit-exact ----
+    pl, rg = R.export_binning(n, H, W, binning, img)
+    _exact_forward(ref, n, radii, is_used, pl, rg)
+
+    # ---- image: L1 / PSNR (bit-identical images pass outright; otherwise on the recorded sample of pixel rows) ----
+    for name, x in (("color", color), ("depth", depth)):
+        if not ref.same(name, _pix(x)):
+            _, a, b, _ = ref.sample(name, _pix(x))
+            assert np.abs(a - b).mean() <= 1e-4 and np.abs(a - b).max() <= 2e-3, name
+            if name == "color":
+                assert psnr(a, b) >= 80.0  # i.e. PSNR against any target differs by << 0.01 dB
+
+    # ---- gradients ----
+    e = torch.Tensor([])
+    ours = R.rasterize_gaussians_backward(bg, t["means3D"], radii, e, t["scales"], t["rotations"], 1.0, e, c["viewmatrix"],
+                                          c["projmatrix"], c["tanfovx"], c["tanfovy"], gdep, gcol, t["shs"], degree,
+                                          c["campos"], geom, n, binning, img, False)
+    for name, o in zip(GRADS, ours):
+        err = ref.rel_err("grad_" + name, _np(o))
+        assert err <= 2e-4, f"grad {name}: rel err {err}"
+
+
+OPTION_CASES = [(2, 0.7, (250, 190)), (1, 1.6, (96, 64)), (0, 1.0, (17, 33))]
+
+
+@pytest.mark.parametrize("active_degree,scale_modifier,size", OPTION_CASES)
+def test_options_vs_reference_cuda(cuda, active_degree, scale_modifier, size):
+    """SH table larger than the active degree (the SLAM raises active_sh_degree over time), scale_modifier != 1, image
+    sizes that are not multiples of the 16x16 tile, non-zero background."""
+    from gs_icp_slam_b200 import rasterizer as R
+
+    t, c, bg, gcol, gdep = case_options(cuda, active_degree, size)
+    W, H = size
+    e = torch.Tensor([])
+    n, depth, color, radii, is_used, geom, binning, img = R.rasterize_gaussians(
+        bg, t["means3D"], e, t["opacities"], t["scales"], t["rotations"], scale_modifier, e, c["viewmatrix"], c["projmatrix"],
+        c["tanfovx"], c["tanfovy"], H, W, t["shs"], active_degree, c["campos"], False, False)
+    ref = _gold(f"opt_{active_degree}")
+    assert n > 0
+    pl, rg = R.export_binning(n, H, W, binning, img)
+    _exact_forward(ref, n, radii, is_used, pl, rg, color, depth)  # bit-identical images
+    ours = R.rasterize_gaussians_backward(bg, t["means3D"], radii, e, t["scales"], t["rotations"], scale_modifier, e,
+                                          c["viewmatrix"], c["projmatrix"], c["tanfovx"], c["tanfovy"], gdep, gcol, t["shs"],
+                                          active_degree, c["campos"], geom, n, binning, img, False)
+    for name, o in zip(GRADS, ours):
+        assert ref.rel_err("grad_" + name, _np(o)) <= 2e-4, name
+    # SH coefficients above the active degree receive no gradient
+    assert float(ours[5][:, (active_degree + 1) ** 2:, :].abs().max()) == 0.0
+    # mark_visible (rasterize_points.cu:208-227) = the near-plane test of the forward pass
+    vis = R.mark_visible(t["means3D"], c["viewmatrix"], c["projmatrix"])
+    assert bool((vis | (radii == 0)).all())
+
+
+def test_degenerate_gaussians_vs_reference_cuda(cuda):
+    """Finite but extreme inputs: zero scales (only the 0.3 px low-pass is left), 1 km scales (the rectangle is the whole
+    screen), saturated and vanishing opacities, Gaussians exactly on the near plane and on the camera centre."""
+    from gs_icp_slam_b200 import rasterizer as R
+
+    t, c, bg, gcol, gdep, a = case_degenerate(cuda)
+    W, H = 200, 152
+    n, depth, color, radii, is_used, geom, binning, img = _ours(t, c, H, W, bg)
+    ref = _gold("degenerate")
+    pl, rg = R.export_binning(n, H, W, binning, img)
+    _exact_forward(ref, n, radii, is_used, pl, rg, color, depth)  # bit patterns (robust to inf / nan)
     e = torch.Tensor([])
     ours = R.rasterize_gaussians_backward(bg, t["means3D"], radii, e, t["scales"], t["rotations"], 1.0, e, c["viewmatrix"],
                                           c["projmatrix"], c["tanfovx"], c["tanfovy"], gdep, gcol, t["shs"], 0, c["campos"],
                                           geom, n, binning, img, False)
-    rgrad = ref.backward(gcol, gdep)
-    for name, o in zip(["means2D", "colors", "opacity", "means3D", "cov3D", "sh", "scales", "rotations"], ours):
-        a_, b_ = o.cpu().numpy(), rgrad[name].cpu().numpy()
+    needles = set(a[12:16].tolist())
+    for name, o in zip(GRADS, ours):
+        a_ = _np(o)
+        assert ref.finite_matches("grad_" + name, a_), name
+        # every modified Gaussian is among the recorded rows (tests/golden/make_raster_ref_cases_golden.py)
+        rows, x, b_, smax = ref.sample("grad_" + name, a_)
         fin = np.isfinite(b_)
-        assert np.array_equal(np.isfinite(a_), fin), name
-        d = np.where(fin, np.abs(a_.astype(np.float64) - b_), 0.0).reshape(a_.shape[0], -1).max(1)
-        scale_ = np.abs(np.where(fin, b_, 0.0)).reshape(a_.shape[0], -1).max(1)
+        d = np.where(fin, np.abs(x.astype(np.float64) - b_), 0.0).max(1)
+        scale_ = np.abs(np.where(fin, b_, 0.0)).max(1)
         # the 1 km x 2 cm "needles" produce gradients of 1e9..1e10 out of terms that cancel to 7 digits: float32 noise
         # in both implementations (their forward output is still bit-identical); only their finiteness is compared
-        d[a[12:16].cpu().numpy()] = 0.0
-        bad = np.flatnonzero(d > 5e-4 * np.maximum(scale_, 1e-3 * scale_.max()))
+        d[[k for k, r in enumerate(rows) if int(r) in needles]] = 0.0
+        bad = np.flatnonzero(d > 5e-4 * np.maximum(scale_, 1e-3 * smax))
         slots = {int(v): k for k, v in enumerate(a.tolist())}
-        assert len(bad) == 0, (name, [(int(i), slots.get(int(i), -1), float(d[i]), float(scale_[i])) for i in bad[:8]])
-    ref.free()
+        assert len(bad) == 0, (name, [(int(rows[i]), slots.get(int(rows[i]), -1), float(d[i]), float(scale_[i])) for i in bad[:8]])
 
 
 def test_tile_shards_partition_the_frame(cuda):
@@ -201,65 +306,40 @@ def test_precomputed_colors_and_cov3d_vs_reference_cuda(cuda):
     """The alternative inputs of GaussianRasterizer.forward: colors_precomp instead of SHs, cov3D_precomp instead of
     scale/rotation (DGR/diff_gaussian_rasterization/__init__.py:189-222)."""
     from gs_icp_slam_b200 import rasterizer as R
-    from oracle import ref_cuda
 
-    if not ref_cuda.available():
-        pytest.skip("oracle/_ref/libref_cuda.so not built")
-    P, (W, H) = 30000, (320, 240)
-    g, cm, t, c, cam = scene_tensors(P, 23, cuda, size=(W, H))
-    gen = torch.Generator(device="cpu").manual_seed(1)
-    colors = torch.rand((P, 3), generator=gen).to(cuda)
-    # Sigma = Rm diag(s^2) Rm^T with Rm the rotation of the (x,y,z,w) quaternion (forward.cu:122-168), upper triangle
-    q, s = t["rotations"].double(), t["scales"].double()
-    x, y, z, w = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
-    Rm = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y), 2 * (x * y + w * z),
-                      1 - 2 * (x * x + z * z), 2 * (y * z - w * x), 2 * (x * z - w * y), 2 * (y * z + w * x),
-                      1 - 2 * (x * x + y * y)], 1).view(P, 3, 3)
-    Sg = Rm @ torch.diag_embed(s * s) @ Rm.transpose(1, 2)
-    cov = torch.stack([Sg[:, 0, 0], Sg[:, 0, 1], Sg[:, 0, 2], Sg[:, 1, 1], Sg[:, 1, 2], Sg[:, 2, 2]], 1).float().contiguous()
-    bg = torch.tensor([0.2, 0.1, 0.4], device=cuda)
+    W, H = 320, 240
+    t, c, bg, colors, cov, gcol, gdep = case_precomputed(cuda)
     n, depth, color, radii, is_used, geom, binning, img = _ours(t, c, H, W, bg, 0, colors=colors, cov=cov)
-    ref = ref_cuda.RefRaster(bg, t["means3D"], None, colors, t["opacities"].reshape(-1), None, None, cov, c["viewmatrix"],
-                             c["projmatrix"], c["campos"], c["tanfovx"], c["tanfovy"], H, W, 0)
-    assert n == ref.num_rendered and torch.equal(radii, ref.radii)
-    assert torch.equal(color, ref.color) and torch.equal(depth, ref.depth)
-    gcol = torch.randn((3, H, W), generator=gen).to(cuda)
-    gdep = torch.randn((1, H, W), generator=gen).to(cuda)
+    ref = _gold("precomputed")
+    assert n == int(ref.full("num_rendered"))
+    ref.exact("radii", _np(radii))
+    ref.exact("color", _pix(color))
+    ref.exact("depth", _pix(depth))
     e = torch.Tensor([])
     ours = R.rasterize_gaussians_backward(bg, t["means3D"], radii, colors, e, e, 1.0, cov, c["viewmatrix"], c["projmatrix"],
                                           c["tanfovx"], c["tanfovy"], gdep, gcol, e, 0, c["campos"], geom, n, binning, img,
                                           False)
-    rg = ref.backward(gcol, gdep)
-    for name, o in zip(["means2D", "colors", "opacity", "means3D", "cov3D"], ours[:5]):
-        assert rel_err(o.cpu().numpy(), rg[name].cpu().numpy()) <= 2e-4, name
+    for name, o in zip(GRADS[:5], ours[:5]):
+        assert ref.rel_err("grad_" + name, _np(o)) <= 2e-4, name
     assert ours[5].numel() == 0 and float(ours[6].abs().sum()) == 0 and float(ours[7].abs().sum()) == 0
-    ref.free()
 
 
-@pytest.mark.parametrize("P,lo,hi", [(9000, 4096, 16384), (40000, 16384, 1 << 30)])
+CROWDED_CASES = [(9000, 4096, 16384), (40000, 16384, 1 << 30)]
+
+
+@pytest.mark.parametrize("P,lo,hi", CROWDED_CASES)
 def test_crowded_tile_uses_segmented_sort_fallback(cuda, P, lo, hi):
     """Crowded tiles: 1024..16384 instances go through the 1024-thread shared-memory sort, more than 16384 hand the whole
     frame over to the segmented radix sort; either way the sorted list must equal the reference's, including ties on equal
     depth (duplicated Gaussians)."""
     from gs_icp_slam_b200 import rasterizer as R
-    from oracle import ref_cuda
 
-    if not ref_cuda.available():
-        pytest.skip("oracle/_ref/libref_cuda.so not built")
-    g, cm, t, c, cam = scene_tensors(P, 31, cuda, size=(160, 120))
-    # pull every Gaussian towards a point 2 m in front of the camera so that a few tiles hold thousands of instances
-    centre = c["campos"] + 2.0 * c["viewmatrix"][:3, 2]  # viewmatrix = (world->view)^T: column 2 is the optical axis
-    t["means3D"] = (centre + 0.02 * (t["means3D"] - t["means3D"].mean(0))).contiguous()
-    t["means3D"][100:200] = t["means3D"][300:400]  # exact duplicates: equal depth keys, order decided by the index
-    bg = torch.zeros(3, device=cuda)
+    t, c, bg = case_crowded(cuda, P)
     n, depth, color, radii, is_used, geom, binning, img = _ours(t, c, 120, 160, bg)
-    ref = _ref(t, c, 120, 160, bg)
     pl, rg = R.export_binning(n, 120, 160, binning, img)
-    rpl, rrg = ref.export()
     assert lo < int((rg[:, 1] - rg[:, 0]).max()) <= hi, "scene does not exercise the intended sort path"
-    assert n == ref.num_rendered and torch.equal(rg, rrg) and torch.equal(pl, rpl)
-    assert torch.equal(color, ref.color) and torch.equal(depth, ref.depth)
-    ref.free()
+    ref = _gold(f"crowded_{P}")
+    _exact_forward(ref, n, None, None, pl, rg, color, depth)
 
 
 def test_cull_is_exact(cuda):
@@ -349,55 +429,30 @@ def test_empty_and_offscreen(cuda):
     assert torch.allclose(out[1], torch.full((1, 48, 64), 15.0, device=cuda))
 
 
-@pytest.mark.parametrize("P,size,degree,seed", [(100000, (640, 480), 0, 3), (30000, (333, 211), 3, 5), (300000, (640, 480), 0, 3)])
+EXT_CASES = [(100000, (640, 480), 0, 3), (30000, (333, 211), 3, 5), (300000, (640, 480), 0, 3)]
+
+
+@pytest.mark.parametrize("P,size,degree,seed", EXT_CASES)
 def test_autograd_vs_reference_torch_extension(cuda, P, size, degree, seed):
     """Drop-in parity at the Python API: this repo's diff_gaussian_rasterization against the REFERENCE's own package
-    (unmodified sources built through their setup.py into oracle/_ref/site — rasterize_points.cu + ext.cpp, the stock
-    path), same module call, same autograd.backward; includes a second backward on a retained graph and sh_degree below
-    the SH table size."""
-    from oracle import ref_ext
-
-    if not ref_ext.available():
-        pytest.skip("oracle/_ref/site not built (oracle/build_ref_ext.sh needs /root/reference)")
+    (unmodified sources built through their setup.py — rasterize_points.cu + ext.cpp, the stock path), same module call,
+    same autograd.backward; includes a second backward on a retained graph (against the reference's first: both of its
+    passes sum the same terms) and sh_degree below the SH table size."""
     import diff_gaussian_rasterization as ours
 
-    ref = ref_ext.diff_gaussian_rasterization()
-    assert ref.GaussianRasterizer is not ours.GaussianRasterizer
-    g, cm, t, c, cam = scene_tensors(P, seed, cuda, sh_degree=degree, size=size)
+    t, c, bg, gcol, gdep, active = case_ext(cuda, P, size, degree, seed)
     W, H = size
-    bg = torch.tensor([0.1, 0.2, 0.3], device=cuda)
-    gen = torch.Generator(device="cpu").manual_seed(11)
-    gcol = torch.randn((3, H, W), generator=gen).to(cuda)
-    gdep = torch.randn((1, H, W), generator=gen).to(cuda)
-    active = max(degree - 1, 0) if degree == 3 else degree  # degree-3 table rendered at degree 2: the tail gets zero grads
-    res = {}
-    for name, mod in (("ours", ours), ("ref", ref)):
-        p = {k: v.detach().clone().requires_grad_(True) for k, v in t.items()}
-        m2 = torch.zeros_like(p["means3D"], requires_grad=True)
-        rs = mod.GaussianRasterizationSettings(H, W, c["tanfovx"], c["tanfovy"], bg, 1.0, c["viewmatrix"], c["projmatrix"],
-                                               active, c["campos"], False, False)
-        depth, color, radii, is_used = mod.GaussianRasterizer(rs)(means3D=p["means3D"], means2D=m2, opacities=p["opacities"],
-                                                                  shs=p["shs"], scales=p["scales"], rotations=p["rotations"])
-        loss = (color * gcol).sum() + (depth * gdep).sum()
-        loss.backward(retain_graph=True)
-        g1 = {k: v.grad.clone() for k, v in p.items()}
-        g1["means2D"] = m2.grad.clone()
-        for v in p.values():
-            v.grad = None
-        m2.grad = None
-        loss.backward()  # second backward on the same saved state
-        g2 = {k: v.grad.clone() for k, v in p.items()}
-        res[name] = (depth.detach(), color.detach(), radii, is_used, g1, g2)
-    o, r = res["ours"], res["ref"]
-    assert torch.equal(o[2], r[2]) and torch.equal(o[3], r[3])
-    assert torch.equal(o[0], r[0]) and torch.equal(o[1], r[1])  # images bit-identical
-    for k in r[4]:
-        assert rel_err(o[4][k].cpu().numpy(), r[4][k].cpu().numpy()) <= 2e-4, k
-    for k in r[5]:
-        assert rel_err(o[5][k].cpu().numpy(), r[5][k].cpu().numpy()) <= 2e-4, ("second backward", k)
+    depth, color, radii, is_used, g1, g2 = run_ext(ours, t, c, H, W, bg, gcol, gdep, active)
+    ref = _gold(f"ext_{P}_{degree}_{seed}")
+    ref.exact("radii", _np(radii))
+    ref.exact("is_used", _np(is_used))
+    ref.exact("depth", _pix(depth))  # images bit-identical
+    ref.exact("color", _pix(color))
+    for k in EXT_GRADS:
+        assert ref.rel_err("grad_" + k, _np(g1[k])) <= 2e-4, k
+        assert ref.rel_err("grad_" + k, _np(g2[k])) <= 2e-4, ("second backward", k)
     if degree == 3:
-        assert float(o[4]["shs"][:, (active + 1) ** 2:].abs().max()) == 0.0
-
+        assert float(g1["shs"][:, (active + 1) ** 2:].abs().max()) == 0.0
 
 
 @pytest.mark.parametrize("variant", [0, 1])
@@ -405,10 +460,7 @@ def test_backward_staging_variants_vs_reference_extension(cuda, variant):
     """render_backward_kernel ships in two launch configurations (256-entry staging / 3 CTAs per SM, the default, and 128-entry
     staging / 4 CTAs per SM).  Each one must match the reference extension's gradients on its own."""
     from gs_icp_slam_b200 import _lib
-    from oracle import ref_ext
 
-    if not ref_ext.available():
-        pytest.skip("oracle/_ref/site not built (oracle/build_ref_ext.sh needs /root/reference)")
     _lib.lib.gsicp_test_set_bwd_variant(variant)
     try:
         test_autograd_vs_reference_torch_extension(cuda, 100000, (640, 480), 0, 3)

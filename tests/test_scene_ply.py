@@ -1,7 +1,8 @@
 """N4 (SURVEY.md §8f): scene.ply written by gs_icp_slam_b200.map_table — byte layout, round trip, and byte-for-byte equality
-with the reference's own GaussianModel.save_ply (scene/gaussian_model.py:619-636, imported unmodified from the installed copy
-under oracle/_ref/gs_icp_slam; the `plyfile` package it calls is absent from this image and replaced by oracle/stubs/plyfile.py,
-which only serialises the structured array the reference hands it)."""
+with the reference's own GaussianModel.save_ply (scene/gaussian_model.py:619-636, run unmodified with its `plyfile` import
+served by oracle/stubs/plyfile.py, which only serialises the structured array the reference hands it; the digest of its
+output is stored in tests/golden/scene_ply_ref.npz)."""
+import hashlib
 import os
 import sys
 
@@ -10,7 +11,6 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SLAM = os.path.join(ROOT, "oracle", "_ref", "gs_icp_slam")
 
 
 def _params(n, degree, seed=0):
@@ -49,13 +49,10 @@ def test_layout_and_round_trip(tmp_path, n, degree):
         read_scene_ply(path, degree + 1)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_SLAM), reason="oracle/_ref/gs_icp_slam not installed (oracle/install_ref_slam.sh)")
-@pytest.mark.parametrize("degree", [0, 3])
-def test_same_bytes_as_reference_save_ply(tmp_path, degree):
-    from gs_icp_slam_b200.map_table import write_scene_ply
-
+def reference_save_ply(ref_slam, out_dir, degree):
+    """Writes scene.ply through the reference's own GaussianModel.save_ply (tests/golden/make_reference_cpu_golden.py)."""
     saved_path, saved_mods = list(sys.path), set(sys.modules)
-    sys.path[:0] = [ROOT, os.path.join(ROOT, "oracle", "stubs"), REF_SLAM]
+    sys.path[:0] = [ROOT, os.path.join(ROOT, "oracle", "stubs"), ref_slam]
     try:
         from scene.gaussian_model import GaussianModel  # the reference's class, unmodified
 
@@ -63,12 +60,22 @@ def test_same_bytes_as_reference_save_ply(tmp_path, degree):
         gm = GaussianModel(degree)
         gm._xyz, gm._features_dc, gm._features_rest = p["xyz"], p["features_dc"], p["features_rest"]
         gm._opacity, gm._scaling, gm._rotation = p["opacity"], p["scaling"], p["rotation"]
-        ref_path, our_path = str(tmp_path / "ref" / "scene.ply"), str(tmp_path / "ours" / "scene.ply")
-        gm.save_ply(ref_path)
-        write_scene_ply(our_path, **p)
-        assert open(ref_path, "rb").read() == open(our_path, "rb").read()
+        path = os.path.join(out_dir, "ref", "scene.ply")
+        gm.save_ply(path)
+        return path
     finally:
         sys.path[:] = saved_path
         for k in list(sys.modules):
             if k not in saved_mods and k.split(".")[0] in ("scene", "utils", "arguments", "plyfile", "open3d", "rerun", "torchmetrics"):
                 del sys.modules[k]
+
+
+@pytest.mark.parametrize("degree", [0, 3])
+def test_same_bytes_as_reference_save_ply(tmp_path, degree):
+    """Our file against the SHA-256 of the bytes the reference's save_ply writes for the same parameters."""
+    from gs_icp_slam_b200.map_table import write_scene_ply
+
+    our_path = str(tmp_path / "ours" / "scene.ply")
+    write_scene_ply(our_path, **_params(300, degree, seed=3))
+    ref_sha = np.load(os.path.join(ROOT, "tests", "golden", "scene_ply_ref.npz"))[f"degree{degree}"].tobytes()
+    assert hashlib.sha256(open(our_path, "rb").read()).digest() == ref_sha
