@@ -85,6 +85,7 @@ _sig("gsicp_mark_visible", i32, [i32, vp, vp, vp, vp, vp])
 _sig("gsicp_test_set_render_cull", None, [i32])
 _sig("gsicp_test_set_bwd_variant", None, [i32])
 _sig("gsicp_test_preload_kernels", i32, [])
+_sig("gsicp_test_grid_meta", i32, [vp, i32, C.POINTER(C.c_float), C.POINTER(C.c_int)])
 _sig("gsicp_dist2", i32, [i32, vp, vp, vp])
 
 _sig("gsicp_gicp_create", vp, [])

@@ -2041,3 +2041,30 @@ extern "C" int gsicp_test_preload_kernels(void) {
   for (const void* f : fns) GSICP_CUDA(cudaFuncGetAttributes(&fa, f));
   return gsicp::comm_preload_kernels();
 }
+
+// Test hook (tests/test_grid_search_gpu.py): the geometry of a search grid, read back so that a test can check that its
+// float32 model of the grid (tests/grid_model.py) bins points exactly as the device does.  h: a GICP handle (which = 0:
+// target grid, 1: source grid) or null for the grid of the last distCUDA2 call.  out_f = {ox, oy, oz, cell, inv_cell},
+// out_i = {nx, ny, nz, ncells}.  Read-only; GSICP_ESTATE when that grid has not been built.
+namespace gsicp { int dist2_grid_meta(GridMeta* out); }
+extern "C" int gsicp_test_grid_meta(gsicp_gicp* h, int which, float out_f[5], int out_i[4]) {
+  if (!out_f || !out_i || (h && which != 0 && which != 1)) {
+    set_error("gsicp_test_grid_meta: bad arguments");
+    return GSICP_EINVAL;
+  }
+  GridMeta m;
+  if (h) {
+    const Cloud& c = which == 0 ? h->tgt : h->src;
+    if (c.grid_stale || c.n <= 0) {
+      set_error("gsicp_test_grid_meta: that grid has not been built");
+      return GSICP_ESTATE;
+    }
+    GSICP_CUDA(cudaStreamSynchronize(h->stream));
+    GSICP_CUDA(cudaMemcpy(&m, c.grid.meta_buf.ptr, sizeof(GridMeta), cudaMemcpyDeviceToHost));
+  } else if (int e = gsicp::dist2_grid_meta(&m)) {
+    return e;
+  }
+  out_f[0] = m.ox; out_f[1] = m.oy; out_f[2] = m.oz; out_f[3] = m.cell; out_f[4] = m.inv_cell;
+  out_i[0] = m.nx; out_i[1] = m.ny; out_i[2] = m.nz; out_i[3] = m.ncells;
+  return GSICP_OK;
+}

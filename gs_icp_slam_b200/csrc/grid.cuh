@@ -127,15 +127,24 @@ static __global__ void grid_setup_kernel(const unsigned int* bb, int n, int max_
   *meta = grid_choose(lo, hi, n, max_cells);
 }
 
+// Coordinate of the lower face of cell k along one axis: o + k * cell, rounded twice whatever the translation unit's fma
+// contraction setting, so that binning (grid_cell_of) and the stopping bound (ring_bound) agree on where every face is.
+__device__ __forceinline__ float grid_face(float o, int k, float cell) { return __fadd_rn(o, __fmul_rn((float)k, cell)); }
+
+// Cell of x along one axis.  The floor of (x - o) * inv_cell can land one cell off near a face (its two roundings differ
+// from grid_face's, by up to ~1e-3 cell at cell index ~4000 when the box straddles 0); it is corrected against grid_face,
+// so every binned point satisfies grid_face(i) <= x < grid_face(i + 1) except beyond the outer faces of the grid.
+__device__ __forceinline__ int grid_axis_cell(float x, float o, float inv_cell, float cell, int n) {
+  int c = (int)floorf(__fmul_rn(__fsub_rn(x, o), inv_cell));
+  c = min(max(c, 0), n - 1);  // NaN/inf -> clamp (the int conversion of NaN is 0 on the device)
+  if (x < grid_face(o, c, cell)) c = max(c - 1, 0);
+  else if (x >= grid_face(o, c + 1, cell)) c = min(c + 1, n - 1);
+  return c;
+}
+
 __device__ __forceinline__ int3 grid_cell_of(const GridMeta& m, float x, float y, float z) {
-  int cx = (int)floorf((x - m.ox) * m.inv_cell);
-  int cy = (int)floorf((y - m.oy) * m.inv_cell);
-  int cz = (int)floorf((z - m.oz) * m.inv_cell);
-  // NaN/inf -> clamp (the int conversion of NaN is 0 on the device)
-  cx = min(max(cx, 0), m.nx - 1);
-  cy = min(max(cy, 0), m.ny - 1);
-  cz = min(max(cz, 0), m.nz - 1);
-  return make_int3(cx, cy, cz);
+  return make_int3(grid_axis_cell(x, m.ox, m.inv_cell, m.cell, m.nx), grid_axis_cell(y, m.oy, m.inv_cell, m.cell, m.ny),
+                   grid_axis_cell(z, m.oz, m.inv_cell, m.cell, m.nz));
 }
 
 static __global__ void grid_count_kernel(int n, const float* __restrict__ xyz, const GridMeta* __restrict__ meta,
@@ -499,18 +508,21 @@ __device__ __forceinline__ uint32_t ring_element(const RingCursor& c, uint32_t t
   return sb + (t - se);
 }
 
+// Squared distance below which a candidate is certainly nearer than every point outside the block of Chebyshev radius r
+// around c0.  Every point binned outside the block lies beyond one of its faces as grid_face places them (grid_cell_of's
+// invariant), so its true distance to q exceeds the exact q - face gap along that axis.  The shrink covers only the
+// rounding of that subtraction (<= 2^-24 relative) and of the candidates' fp32 squared distances (a few ulp).
 __device__ __forceinline__ float ring_bound(const GridMeta& m, int3 c0, int r, float qx, float qy, float qz, bool& all) {
   all = (c0.x - r <= 0 && c0.y - r <= 0 && c0.z - r <= 0 && c0.x + r >= m.nx - 1 && c0.y + r >= m.ny - 1 && c0.z + r >= m.nz - 1);
   float bound = FLT_MAX;
-  if (c0.x - r > 0) bound = fminf(bound, qx - (m.ox + (c0.x - r) * m.cell));
-  if (c0.x + r < m.nx - 1) bound = fminf(bound, (m.ox + (c0.x + r + 1) * m.cell) - qx);
-  if (c0.y - r > 0) bound = fminf(bound, qy - (m.oy + (c0.y - r) * m.cell));
-  if (c0.y + r < m.ny - 1) bound = fminf(bound, (m.oy + (c0.y + r + 1) * m.cell) - qy);
-  if (c0.z - r > 0) bound = fminf(bound, qz - (m.oz + (c0.z - r) * m.cell));
-  if (c0.z + r < m.nz - 1) bound = fminf(bound, (m.oz + (c0.z + r + 1) * m.cell) - qz);
-  // conservative: shrink by the fp32 error of the face coordinates and of the distances
-  const float safe = fmaxf(bound, 0.f) * (1.0f - 1e-5f) - 1e-6f * m.cell;
-  return safe > 0.f ? safe * safe * (1.0f - 1e-5f) : -1.f;  // squared; -1: no conclusion possible yet
+  if (c0.x - r > 0) bound = fminf(bound, __fsub_rn(qx, grid_face(m.ox, c0.x - r, m.cell)));
+  if (c0.x + r < m.nx - 1) bound = fminf(bound, __fsub_rn(grid_face(m.ox, c0.x + r + 1, m.cell), qx));
+  if (c0.y - r > 0) bound = fminf(bound, __fsub_rn(qy, grid_face(m.oy, c0.y - r, m.cell)));
+  if (c0.y + r < m.ny - 1) bound = fminf(bound, __fsub_rn(grid_face(m.oy, c0.y + r + 1, m.cell), qy));
+  if (c0.z - r > 0) bound = fminf(bound, __fsub_rn(qz, grid_face(m.oz, c0.z - r, m.cell)));
+  if (c0.z + r < m.nz - 1) bound = fminf(bound, __fsub_rn(grid_face(m.oz, c0.z + r + 1, m.cell), qz));
+  const float safe = __fsub_rn(__fmul_rn(fmaxf(bound, 0.f), 1.0f - 1e-5f), __fmul_rn(1e-6f, m.cell));
+  return safe > 0.f ? __fmul_rn(__fmul_rn(safe, safe), 1.0f - 1e-5f) : -1.f;  // squared; -1: no conclusion possible yet
 }
 
 // k-NN, k <= 32.  On return lane i < kth holds the i-th nearest (d2, id), ordered by (d2, id); the other lanes

@@ -24,6 +24,18 @@ dist2_kernel(GridView g, const float* __restrict__ xyz, float* __restrict__ out)
 static DeviceGrid g_dist2_grid;
 static std::mutex g_dist2_mu;
 
+// Geometry of the grid of the last distCUDA2 call (test hook gsicp_test_grid_meta); GSICP_ESTATE before the first call.
+int dist2_grid_meta(GridMeta* out) {
+  std::lock_guard<std::mutex> lock(g_dist2_mu);
+  if (g_dist2_grid.n <= 0 || !g_dist2_grid.meta_buf.ptr) {
+    set_error("gsicp_test_grid_meta: distCUDA2 has not built a grid yet");
+    return GSICP_ESTATE;
+  }
+  GSICP_CUDA(cudaDeviceSynchronize());
+  GSICP_CUDA(cudaMemcpy(out, g_dist2_grid.meta_buf.ptr, sizeof(GridMeta), cudaMemcpyDeviceToHost));
+  return GSICP_OK;
+}
+
 }  // namespace gsicp
 
 using namespace gsicp;
