@@ -138,6 +138,11 @@ _sig("gsicp_mapping_loss_work_bytes", C.c_size_t, [i32, i32])
 _sig("gsicp_mapping_loss_forward", i32, [i32, i32, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float, i32, vp, vp, vp, vp, vp])
 _sig("gsicp_mapping_loss_backward", i32, [i32, i32, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float, i32, vp, vp, vp, vp, vp])
 _sig("gsicp_gicp_last_timing", i32, [vp, vp])
+_sig("gsicp_vgicp_create", vp, [])
+_sig("gsicp_vgicp_set_resolution", i32, [vp, C.c_double])
+_sig("gsicp_vgicp_set_neighbor_search", i32, [vp, i32])
+_sig("gsicp_vgicp_voxel_count", i32, [vp])
+_sig("gsicp_vgicp_get_voxels", i32, [vp, vp, vp])
 
 # BOUND lists every bound symbol; tests/test_abi.py checks include/gsicp_b200.h against it.
 

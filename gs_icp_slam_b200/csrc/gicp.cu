@@ -29,16 +29,10 @@
 
 #include "grid.cuh"
 #include "comm.cuh"
+#include "gicp_reduce.cuh"
+#include "vgicp.cuh"
 
 namespace gsicp {
-
-constexpr int kRed = 28;       // 21 (upper triangle of H, row-major) + 6 (b) + 1 (error)
-constexpr int kLinBlock = 128;
-
-struct PoseD {  // pose in both precisions, passed by value
-  double R[3][3], t[3];
-  float Rf[3][3], tf[3];
-};
 
 // ------------------------------------------------------------------------------------------------
 // covariance kernel
@@ -221,81 +215,8 @@ __global__ void cov_from_qs_kernel(int n, const float* __restrict__ rots, const 
 }
 
 // ------------------------------------------------------------------------------------------------
-// linearize / error kernels
+// linearize / error kernels (block reduction: gicp_reduce.cuh)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// block-level reduction of NV doubles per thread into partial[blockIdx][NV]; the last block to finish
-// sums the partials in block order (deterministic) into out[NV].
-//
-// When `host_out` is non-null (single-GPU runs) the last block also publishes the sums into MAPPED PINNED host memory and
-// then bumps a sequence word the host spins on: the result reaches the LM loop without a D2H memcpy or a
-// cudaStreamSynchronize round trip (two driver calls and a thread wake-up per launch otherwise).
-template <int NV>
-__device__ __forceinline__ void block_reduce_finalize(double* v, double* __restrict__ partial, double* __restrict__ out,
-                                                      unsigned int* __restrict__ counter, double* host_out = nullptr,
-                                                      volatile unsigned long long* host_seq = nullptr,
-                                                      unsigned long long seq = 0, CommView comm = CommView(),
-                                                      unsigned long long xseq = 0) {
-  __shared__ double s_red[kLinBlock / 32][NV];
-  __shared__ double s_tot[NV];
-  __shared__ bool s_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < NV; k++) {
-    const double r = warp_sum_d(v[k]);
-    if (lane == 0) s_red[warp][k] = r;
-  }
-  __syncthreads();
-  if (threadIdx.x < NV) {
-    double r = 0.0;
-#pragma unroll
-    for (int w = 0; w < kLinBlock / 32; w++) r += s_red[w][threadIdx.x];
-    partial[(size_t)blockIdx.x * NV + threadIdx.x] = r;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned int done = atomicAdd(counter, 1u);
-    s_last = (done == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    if (threadIdx.x < NV) {
-      double r = 0.0;
-      for (unsigned int b = 0; b < gridDim.x; b++) r += partial[(size_t)b * NV + threadIdx.x];
-      s_tot[threadIdx.x] = r;
-    }
-    __syncthreads();
-    if (comm.active()) {
-      // multi-GPU: the last block exchanges this rank's sums with the peers through their segments (comm.cuh) and adds
-      // the world's slots in rank order — the result the host reads is already the global one, bit-identical on all ranks
-      comm_lm_publish(comm, xseq, s_tot, NV);
-      comm_lm_collect(comm, xseq, s_tot, NV);  // a lost peer leaves the local sums in place after the poll budget
-    }
-    if (threadIdx.x < NV) {
-      out[threadIdx.x] = s_tot[threadIdx.x];
-      if (host_out) host_out[threadIdx.x] = s_tot[threadIdx.x];
-    }
-    if (host_out) {
-      __threadfence_system();
-      __syncthreads();  // s_last is block-uniform
-    }
-    if (threadIdx.x == 0) {
-      *counter = 0u;  // ready for the next launch
-      if (host_seq) {
-        *host_seq = seq;
-        __threadfence_system();
-      }
-    }
-  }
-}
-
 struct LinArgs {
   int begin, end;          // source range of this rank
   double max_corr_sq;      // corr_dist_threshold_^2 in double (fgi:271)
@@ -1000,6 +921,13 @@ struct gsicp_gicp {
   double t_cov = 0, t_lin = 0, t_err = 0;
   int n_lin = 0, n_err = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  // FastVGICP handle (gsicp_vgicp_create): voxel map of the target, host-driven LM loop (vgicp.cu)
+  bool vgicp = false;
+  double vox_res = 1.0;          // setResolution (fast_vgicp_impl.hpp:22)
+  int vox_offsets = 1;           // DIRECT1 / DIRECT7 / DIRECT27
+  VoxelMap vox;
+  Iso vox_x0;                    // pose of the last linearize: compute_error uses its voxel pairs and M
+  bool vox_lin = false;
 };
 
 namespace {
@@ -1415,10 +1343,37 @@ int comm_take_seq(gsicp_gicp* h, unsigned long long reserve, unsigned long long*
   return GSICP_OK;
 }
 
-// fgi:296-352.  H may be null (error only).
+// fast_vgicp_impl.hpp:66-70, 120-123: the voxel map of the current target (and its covariances)
+int build_voxelmap(gsicp_gicp* h) {
+  h->vox_lin = false;
+  return voxelmap_build(h->vox, h->tgt.xyz.as<float>(), h->tgt.cov.as<double>(), h->tgt.n, h->vox_res, h->stream);
+}
+
+void drop_voxelmap(gsicp_gicp* h) {  // setInputTarget / swapSourceAndTarget reset the map (fast_vgicp_impl.hpp:46-63)
+  h->vox.n = 0;
+  h->vox_lin = false;
+}
+
+VgicpArgs vgicp_args(gsicp_gicp* h, double* host_out, volatile unsigned long long* host_seq, unsigned long long seq) {
+  VgicpArgs v;
+  v.vox = voxelmap_view(h->vox);
+  v.n_src = h->src.n;
+  v.n_offsets = h->vox_offsets;
+  v.src_xyz = h->src.xyz.as<float>();
+  v.src_cov = h->src.cov.as<double>();
+  v.partial = h->partial.as<double>();
+  v.out = h->red_out.as<double>();
+  v.counter = h->counter.as<unsigned int>();
+  v.host_out = host_out;
+  v.host_seq = host_seq;
+  v.seq = seq;
+  return v;
+}
+
+// fgi:296-352 (VGICP handles: fast_vgicp_impl.hpp:118-180).  H may be null (error only).
 int run_linearize(gsicp_gicp* h, const Iso& x, double H[6][6], double b[6], double* err) {
   if (int e = ensure_lin_buffers(h)) return e;
-  if (h->corr_n != h->src.n) {
+  if (!h->vgicp && h->corr_n != h->src.n) {  // VGICP keeps no point-to-point correspondences
     // sharded runs leave the other ranks' entries untouched: start from "unmatched"
     GSICP_CUDA(cudaMemsetAsync(h->corr.ptr, 0xff, (size_t)(h->src.n + 1) * 4, h->stream));
     GSICP_CUDA(cudaMemsetAsync(h->sqd.ptr, 0, (size_t)(h->src.n + 1) * 4, h->stream));
@@ -1447,15 +1402,21 @@ int run_linearize(gsicp_gicp* h, const Iso& x, double H[6][6], double b[6], doub
   }
   int blocks = (end - begin + kLinBlock - 1) / kLinBlock;
   if (blocks < 1) blocks = 1;
-  if (end > begin)
+  if (end > begin && !h->vgicp)
     if (int e = ensure_grid(h, h->tgt)) return e;
   { ProfScope ps(kProfLinearize, h->stream);
+  if (h->vgicp) {
+    if (int e = vgicp_launch_linearize(vgicp_args(h, a.host_out, a.host_seq, a.seq), make_pose(x), h->stream)) return e;
+    h->vox_x0 = x;
+    h->vox_lin = true;
+  } else {
   if (end > begin) {
     const int nn_blocks = (int)(((size_t)(end - begin) * 32 + 127) / 128);
     GSICP_LAUNCH(correspond_kernel, nn_blocks, 128, 0, h->stream, h->tgt.grid.view(), make_pose(x), begin, end, a.max_corr_sq,
                  a.src_xyz, a.corr, a.sqd);
   }
-  GSICP_LAUNCH(linearize_kernel, blocks, kLinBlock, 0, h->stream, make_pose(x), a); }
+  GSICP_LAUNCH(linearize_kernel, blocks, kLinBlock, 0, h->stream, make_pose(x), a);
+  } }
   if (h->shard_count > 1 && h->reduce) {
     const int rc = h->reduce(h->reduce_user, h->red_out.as<double>(), kRed, (void*)h->stream);
     if (rc != 0) {
@@ -1511,7 +1472,12 @@ int run_error(gsicp_gicp* h, const Iso& x, double* err) {  // fgi:355-378
   int blocks = (end - begin + kLinBlock - 1) / kLinBlock;
   if (blocks < 1) blocks = 1;
   { ProfScope ps(kProfError, h->stream);
-  GSICP_LAUNCH(error_kernel, blocks, kLinBlock, 0, h->stream, make_pose(x), a); }
+  if (h->vgicp) {
+    if (int e = vgicp_launch_error(vgicp_args(h, a.host_out, a.host_seq, a.seq), make_pose(h->vox_x0), make_pose(x), h->stream))
+      return e;
+  } else {
+    GSICP_LAUNCH(error_kernel, blocks, kLinBlock, 0, h->stream, make_pose(x), a);
+  } }
   if (h->shard_count > 1 && h->reduce) {
     const int rc = h->reduce(h->reduce_user, h->red_out.as<double>(), 1, (void*)h->stream);
     if (rc != 0) return GSICP_ECUDA;
@@ -1727,6 +1693,7 @@ void gsicp_gicp_destroy(gsicp_gicp* h) {
   }
   fr(h->corr); fr(h->sqd); fr(h->mahal); fr(h->partial); fr(h->red_out); fr(h->counter); fr(h->staging_dev); fr(h->nn_id); fr(h->nn_d2);
   fr(h->lm_partL); fr(h->lm_partE); fr(h->lm_barrier);
+  voxelmap_free(h->vox);
   if (h->h_lm) cudaFreeHost(h->h_lm);
   if (h->h_red) cudaFreeHost(h->h_red);
   if (h->h_map) cudaFreeHost(h->h_map);
@@ -1753,6 +1720,7 @@ int gsicp_gicp_set_input_source(gsicp_gicp* h, const void* xyz, int n, int is_f3
 }
 int gsicp_gicp_set_input_target(gsicp_gicp* h, const void* xyz, int n, int is_f32) {
   H_CHECK(h);
+  drop_voxelmap(h);
   return set_cloud(h, h->tgt, xyz, n, is_f32, false);
 }
 int gsicp_gicp_set_input_source_device(gsicp_gicp* h, const float* d_xyz, int n) {
@@ -1762,6 +1730,7 @@ int gsicp_gicp_set_input_source_device(gsicp_gicp* h, const float* d_xyz, int n)
 }
 int gsicp_gicp_set_input_target_device(gsicp_gicp* h, const float* d_xyz, int n) {
   H_CHECK(h);
+  drop_voxelmap(h);
   return set_cloud(h, h->tgt, d_xyz, n, 1, true);
 }
 int gsicp_gicp_set_source_filter(gsicp_gicp* h, int nt, const int32_t* f, int n) { H_CHECK(h); return set_filter(h, h->src, nt, f, n); }
@@ -1793,6 +1762,7 @@ int gsicp_gicp_swap_source_and_target(gsicp_gicp* h) {
   std::swap(h->src.zvals, h->tgt.zvals);
   std::swap(h->src.z_n, h->tgt.z_n);
   h->corr_n = -1;
+  drop_voxelmap(h);
   return GSICP_OK;
 }
 
@@ -1826,6 +1796,8 @@ int gsicp_gicp_align(gsicp_gicp* h, const float guess[16], float out[16]) {
     set_error("align: no trackable source points");
     return GSICP_ESTATE;
   }
+  if (h->vgicp)  // FastVGICP::computeTransformation drops the map; the first linearize builds it from the current target
+    if (int e = build_voxelmap(h)) return e;
   Iso x0;
   for (int i = 0; i < 3; i++) {
     for (int j = 0; j < 3; j++) x0.R[i][j] = (double)guess[4 * i + j];
@@ -1838,7 +1810,8 @@ int gsicp_gicp_align(gsicp_gicp* h, const float guess[16], float out[16]) {
   // The persistent kernel (one block per SM) wins where launch / wait latency dominates; above kLmPersistentMax points per
   // rank the phases are throughput-bound and the full-occupancy kernels of the host-driven loop are faster
   // (in a sharded run their last block exchanges through the peers' segments as well: no host-side collective either way).
-  if (!h->host_lm && !h->timing && (h->shard_count <= 1 || h->comm) && (le - lb) <= kLmPersistentMax) {
+  // VGICP always runs the host-driven loop.
+  if (!h->vgicp && !h->host_lm && !h->timing && (h->shard_count <= 1 || h->comm) && (le - lb) <= kLmPersistentMax) {
     // device-resident LM loop: one persistent kernel, zero host round trips inside the loop
     if (h->d_lm) std::memset(h->h_lm->H, 0, sizeof(h->h_lm->H));
     iters = run_align_device(h, x0);
@@ -1970,6 +1943,8 @@ int gsicp_gicp_linearize(gsicp_gicp* h, const double pose[16], double Hout[36], 
   Iso x;
   if (int e = pose_from16(pose, x)) return e;
   if (int e = ready_for_linearize(h)) return e;
+  if (h->vgicp)  // a direct call linearizes against a fresh map of the current target
+    if (int e = build_voxelmap(h)) return e;
   double H[6][6], bb[6], er;
   if (int e = run_linearize(h, x, H, bb, &er)) return e;
   if (Hout) std::memcpy(Hout, H, sizeof(H));
@@ -1983,15 +1958,22 @@ int gsicp_gicp_compute_error(gsicp_gicp* h, const double pose[16], double* err) 
   Iso x;
   if (int e = pose_from16(pose, x)) return e;
   if (int e = ready_for_linearize(h)) return e;
-  if (h->corr_n != h->src.n) {
+  if (h->vgicp ? !h->vox_lin : h->corr_n != h->src.n) {
     set_error("compute_error: run linearize first");
     return GSICP_ESTATE;
   }
   return run_error(h, x, err);
 }
 
+static int refuse_vgicp_shard(gsicp_gicp* h) {
+  if (!h->vgicp) return GSICP_OK;
+  set_error("FastVGICP runs on one GPU");
+  return GSICP_ESTATE;
+}
+
 int gsicp_gicp_set_shard(gsicp_gicp* h, int count, int index, gsicp_allreduce_fn reduce, void* user) {
   H_CHECK(h);
+  if (int e = refuse_vgicp_shard(h)) return e;
   if (count < 1 || index < 0 || index >= count) return GSICP_EINVAL;
   h->shard_count = count; h->shard_index = index; h->reduce = reduce; h->reduce_user = user;
   h->corr_n = -1;
@@ -2000,6 +1982,7 @@ int gsicp_gicp_set_shard(gsicp_gicp* h, int count, int index, gsicp_allreduce_fn
 
 int gsicp_gicp_set_comm(gsicp_gicp* h, gsicp_comm* comm) {
   H_CHECK(h);
+  if (int e = refuse_vgicp_shard(h)) return e;
   if (comm && !comm->connected) {
     set_error("gsicp_gicp_set_comm: the exchange group is not connected");
     return GSICP_ESTATE;
@@ -2018,6 +2001,47 @@ int gsicp_gicp_last_timing(gsicp_gicp* h, double out[5]) {
   H_CHECK(h);
   out[0] = h->t_cov; out[1] = h->t_lin; out[2] = h->t_err; out[3] = h->n_lin; out[4] = h->n_err;
   return GSICP_OK;
+}
+
+// ---- FastVGICP (fast_vgicp.hpp, main.cpp:264-279) ----
+gsicp_gicp* gsicp_vgicp_create(void) {
+  gsicp_gicp* h = gsicp_gicp_create();
+  if (h) h->vgicp = true;
+  return h;
+}
+
+#define VG_CHECK(h)                                            \
+  H_CHECK(h);                                                  \
+  if (!(h)->vgicp) {                                           \
+    set_error("not a FastVGICP handle (gsicp_vgicp_create)"); \
+    return GSICP_ESTATE;                                       \
+  }
+
+int gsicp_vgicp_set_resolution(gsicp_gicp* h, double r) {
+  VG_CHECK(h);
+  if (!(std::isfinite(r) && r > 0.0)) {
+    set_error("voxel resolution must be finite and > 0 (got %g)", r);
+    return GSICP_EINVAL;
+  }
+  h->vox_res = r;  // used from the next map build on (the next align)
+  return GSICP_OK;
+}
+
+int gsicp_vgicp_set_neighbor_search(gsicp_gicp* h, int n_offsets) {
+  VG_CHECK(h);
+  if (n_offsets != 1 && n_offsets != 7 && n_offsets != 27) {
+    set_error("neighbor search: %d offsets (DIRECT1, DIRECT7 or DIRECT27: 1, 7 or 27)", n_offsets);
+    return GSICP_EINVAL;
+  }
+  h->vox_offsets = n_offsets;
+  return GSICP_OK;
+}
+
+int gsicp_vgicp_voxel_count(gsicp_gicp* h) { VG_CHECK(h); return h->vox.n; }
+
+int gsicp_vgicp_get_voxels(gsicp_gicp* h, double* means, double* covs) {
+  VG_CHECK(h);
+  return voxelmap_export(h->vox, means, covs, h->stream);
 }
 
 }  // extern "C"

@@ -21,10 +21,12 @@ def _f32_1d(a):
 class FastGICP:
     """pygicp.FastGICP drop-in.  Picklable like the reference (state is not carried across, main.cpp:183-201)."""
 
+    _create = "gsicp_gicp_create"  # C constructor of the handle kind
+
     def __init__(self):
-        self._h = lib.gsicp_gicp_create()
+        self._h = getattr(lib, self._create)()
         if not self._h:
-            raise _lib.GsicpError("gsicp_gicp_create failed: " + _lib.last_error())
+            raise _lib.GsicpError(f"{self._create} failed: " + _lib.last_error())
         self._stream_ptr = 0  # the handle's stream (0 = legacy default stream)
 
     def _device_input(self, t):
@@ -286,3 +288,37 @@ class FastGICP:
 
             self._cb = _lib.ALLREDUCE_FN(_tramp)
         check(lib.gsicp_gicp_set_shard(self._h, int(count), int(index), self._cb, None))
+
+
+_SEARCH_OFFSETS = {"DIRECT1": 1, "DIRECT7": 7, "DIRECT27": 27}
+
+
+class FastVGICP(FastGICP):
+    """pygicp.FastVGICP drop-in (main.cpp:264-279): a FastGICP whose correspondences are the target's Gaussian voxels
+    (fast_vgicp_impl.hpp, ADDITIVE voxel accumulation).  Every FastGICP method works as on FastGICP, with three
+    differences that follow the reference: max_correspondence_distance is unused, there are no point-to-point
+    correspondences (get_source_correspondence raises), and it runs on one GPU (set_comm / set_shard raise)."""
+
+    _create = "gsicp_vgicp_create"
+
+    def set_resolution(self, resolution):
+        check(lib.gsicp_vgicp_set_resolution(self._h, float(resolution)))
+
+    def set_neighbor_search_method(self, method):
+        if method == "DIRECT_RADIUS":
+            # the reference accepts the name, then abort()s the process in neighbor_offsets at the next align
+            raise ValueError("neighbor search method DIRECT_RADIUS is not supported by FastVGICP")
+        n = _SEARCH_OFFSETS.get(method)
+        if n is None:
+            print(f"error: unknown neighbor search method {method}", file=sys.stderr)  # main.cpp:33-34
+            n = 1
+        check(lib.gsicp_vgicp_set_neighbor_search(self._h, n))
+
+    def get_voxel_mean_cov(self):
+        """(list of (4,) float64 means, list of (4, 4) float64 covariances) of the current voxel map, in the map's key
+        order (the reference's unordered_map order is implementation-defined).  ([], []) before any map exists."""
+        n = check(lib.gsicp_vgicp_voxel_count(self._h))
+        means, covs = np.empty((n, 4)), np.empty((n, 4, 4))
+        if n:
+            check(lib.gsicp_vgicp_get_voxels(self._h, means.ctypes.data, covs.ctypes.data))
+        return list(means), list(covs)

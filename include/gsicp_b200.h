@@ -260,6 +260,23 @@ int gsicp_gicp_set_host_lm(gsicp_gicp* h, int on);
  * [3]=number of linearize launches, [4]=number of compute_error launches. */
 int gsicp_gicp_last_timing(gsicp_gicp*, double out[5]);
 
+/* ---- Voxelized GICP (pygicp.FastVGICP: FG/include/fast_gicp/gicp/fast_vgicp.hpp, main.cpp:264-279) ----------------------
+ * A FastVGICP handle is a gsicp_gicp of the VGICP kind: every gsicp_gicp_* call works on it, except that set_shard and
+ * set_comm return GSICP_ESTATE (it runs on one GPU) and there are no point-to-point correspondences
+ * (get_source_correspondence returns GSICP_ESTATE).  align() builds the ADDITIVE voxel map of the current target and its
+ * covariances, then runs the host-driven LM loop over voxel correspondences; max_correspondence_distance is unused.
+ * The gsicp_vgicp_* calls return GSICP_ESTATE on a plain GICP handle. */
+gsicp_gicp* gsicp_vgicp_create(void);
+/* setResolution; default 1.0.  GSICP_EINVAL unless finite and > 0.  A map whose extent needs more than 2^21 voxels on an
+ * axis is refused by the align / linearize that builds it (GSICP_EINVAL). */
+int gsicp_vgicp_set_resolution(gsicp_gicp*, double resolution);
+/* setNeighborSearchMethod: 1 (DIRECT1, default), 7 (DIRECT7) or 27 (DIRECT27) voxel offsets. */
+int gsicp_vgicp_set_neighbor_search(gsicp_gicp*, int n_offsets);
+/* Voxels of the current map (0 before the first align / linearize and after set_input_target or a swap). */
+int gsicp_vgicp_voxel_count(gsicp_gicp*);
+/* getVoxelMeanCov, in packed-key order: means [V][4] (w = 1), covariances [V][16] row-major with row and column 3 zero. */
+int gsicp_vgicp_get_voxels(gsicp_gicp*, double* means, double* covs);
+
 /* ---- fused mapping loss (SURVEY.md §8f row N2; the caller side of the rasterizer) ----------------------------------
  * Replaces utils/loss_utils.py:17-20 (l1_loss), :38-69 (ssim/_ssim) and their combination in mp_Mapper.py:225-242:
  *   loss = (1-lambda) * mean(|image - gt| where gt != 0) + lambda * (1 - mean(ssim(where(gt != 0, image, 0), gt)))
