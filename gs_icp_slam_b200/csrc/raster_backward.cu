@@ -842,6 +842,35 @@ extern "C" int gsicp_raster_set_comm(gsicp_comm* comm) {
 
 extern "C" size_t gsicp_raster_backward_work_bytes(int P) { (void)P; return 0; }
 
+// Test hook (tests/test_raster_bwd_bound.py): when set, every backward copies the summed [P][12] render moments here, after
+// render_backward and any exchange, before gaussian_backward consumes and re-zeroes them.  Off (null) by default.
+static float* g_moment_tap = nullptr;
+extern "C" void gsicp_test_set_moment_tap(float* d_dst) { g_moment_tap = d_dst; }
+
+// Test hook: the saved forward state the backward replays, through the same carving as the backward itself:
+// the splat records [P][12] = {px, py, conic xx, xy, yy, opacity, cov_zx, cov_yz, r, g, b, depth}, final_T [N] and
+// n_contrib [N].  (point_list and ranges: gsicp_raster_export_binning.)
+extern "C" int gsicp_test_raster_state(const gsicp_raster_args* args, int P, int R, const void* d_geom, const void* d_image,
+                                       float* d_out_splats, float* d_out_final_T, uint32_t* d_out_n_contrib, void* stream_v) {
+  (void)R;
+  if (!args || P < 0 || !d_geom || !d_image) {
+    set_error("gsicp_test_raster_state: bad arguments");
+    return GSICP_EINVAL;
+  }
+  cudaStream_t stream = (cudaStream_t)stream_v;
+  const int W = args->width, H = args->height;
+  const int tiles = ((W + kTile - 1) / kTile) * ((H + kTile - 1) / kTile);
+  const size_t N = (size_t)W * H;
+  GeomState geom = GeomState::from((char*)d_geom, P);
+  ImgState img = ImgState::from((char*)d_image, N, tiles);
+  if (d_out_splats && P > 0)
+    GSICP_CUDA(cudaMemcpyAsync(d_out_splats, geom.splats, sizeof(Splat) * (size_t)P, cudaMemcpyDeviceToDevice, stream));
+  if (d_out_final_T) GSICP_CUDA(cudaMemcpyAsync(d_out_final_T, img.final_T, sizeof(float) * N, cudaMemcpyDeviceToDevice, stream));
+  if (d_out_n_contrib)
+    GSICP_CUDA(cudaMemcpyAsync(d_out_n_contrib, img.n_contrib, sizeof(uint32_t) * N, cudaMemcpyDeviceToDevice, stream));
+  return GSICP_OK;
+}
+
 extern "C" int gsicp_raster_backward(const gsicp_raster_args* args, int num_rendered, const int32_t* d_radii,
                                      const void* d_geom, const void* d_binning, const void* d_image,
                                      const float* d_dL_dout_color, const float* d_dL_dout_depth, float* d_dL_dmeans2D,
@@ -913,6 +942,8 @@ extern "C" int gsicp_raster_backward(const gsicp_raster_args* args, int num_rend
   } else if (shard_count > 1 && g_bwd.fn) {
     if (int e = allreduce_visible_moments(P, d_radii, work, stream)) return e;
   }
+  if (g_moment_tap)
+    GSICP_CUDA(cudaMemcpyAsync(g_moment_tap, work, (size_t)P * kG * sizeof(float), cudaMemcpyDeviceToDevice, stream));
 
   BwdArgs ba;
   ba.P = P; ba.D = args->D; ba.M = args->M;

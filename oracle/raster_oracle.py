@@ -23,12 +23,16 @@ def _load():
     lib.ro_forward.argtypes = [C.POINTER(_Args), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.ro_backward.restype = C.c_int
     lib.ro_backward.argtypes = [C.POINTER(_Args), C.c_void_p, C.c_void_p] + [C.c_void_p] * 10
+    lib.ro_backward_ex.restype = C.c_int
+    lib.ro_backward_ex.argtypes = [C.POINTER(_Args), C.c_void_p, C.c_void_p] + [C.c_void_p] * 12
     lib.ro_num_rendered.restype = C.c_int
     lib.ro_num_rendered.argtypes = [C.c_void_p]
-    for n in ("ro_point_list", "ro_ranges", "ro_n_contrib", "ro_final_T"):
+    for n in ("ro_point_list", "ro_ranges", "ro_n_contrib", "ro_final_T", "ro_means2D", "ro_conic_op", "ro_rgb", "ro_depths"):
         getattr(lib, n).restype = C.c_void_p
         getattr(lib, n).argtypes = [C.c_void_p]
     lib.ro_free.argtypes = [C.c_void_p]
+    lib.ro_moment_reference.restype = C.c_int
+    lib.ro_moment_reference.argtypes = [C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 13
     return lib
 
 
@@ -100,4 +104,96 @@ def forward_backward(scene, cam, H, W, bg, sh_degree=0, scale_modifier=1.0, colo
     finally:
         _lib.ro_free(st)
     r.is_used = r.is_used.astype(bool)
+    return r
+
+
+def _view(ptr, ctype, shape):
+    return np.ctypeslib.as_array(C.cast(ptr, C.POINTER(ctype)), shape)
+
+
+class State:
+    """A forward state of the CPU restatement kept alive for backward replays: the float32 splat records, instance list,
+    tile ranges and per-pixel n_contrib / final_T the backward reads.  `final_T` is a writable view of the state itself.
+    Call free() when done."""
+
+    def __init__(self, scene, cam, H, W, bg, sh_degree=0):
+        global _lib
+        if _lib is None:
+            _lib = _load()
+        self.keep = [_f32(scene["means3D"]), _f32(scene["shs"]), _f32(scene["opacities"]).reshape(-1),
+                     _f32(scene["scales"]), _f32(scene["rotations"]), _f32(cam["viewmatrix"]), _f32(cam["projmatrix"]),
+                     _f32(cam["campos"]), _f32(bg)]
+        means, shs, opac, scales, rots, view, proj, campos, bgc = self.keep
+        P = self.P = means.shape[0]
+        self.H, self.W, self.bg = H, W, bgc
+        self.args = _Args(P, sh_degree, shs.shape[1], W, H, cam["tanfovx"], cam["tanfovy"], 1.0, _p(bgc), _p(means),
+                          _p(shs), None, _p(opac), _p(scales), _p(rots), None, _p(view), _p(proj), _p(campos))
+        self.color = np.zeros((3, H, W), np.float32)
+        self.depth = np.zeros((1, H, W), np.float32)
+        self.radii = np.zeros(P, np.int32)
+        is_used = np.zeros(P, np.uint8)
+        self.st = _lib.ro_forward(C.byref(self.args), self.color.ctypes.data, self.depth.ctypes.data,
+                                  self.radii.ctypes.data, is_used.ctypes.data)
+        R = _lib.ro_num_rendered(self.st)
+        tiles = ((W + 15) // 16) * ((H + 15) // 16)
+        self.point_list = _view(_lib.ro_point_list(self.st), C.c_uint32, (max(R, 1),))[:R]
+        self.ranges = _view(_lib.ro_ranges(self.st), C.c_uint32, (tiles, 2))
+        self.n_contrib = _view(_lib.ro_n_contrib(self.st), C.c_uint32, (H, W))
+        self.final_T = _view(_lib.ro_final_T(self.st), C.c_float, (H, W))
+        m2 = _view(_lib.ro_means2D(self.st), C.c_float, (P, 2))
+        co = _view(_lib.ro_conic_op(self.st), C.c_float, (P, 6))
+        rgb = _view(_lib.ro_rgb(self.st), C.c_float, (P, 3))
+        dep = _view(_lib.ro_depths(self.st), C.c_float, (P,))
+        # the GPU's record layout: {px, py, conic xx, xy, yy, opacity, cov_zx, cov_yz, r, g, b, depth}
+        self.splats = np.ascontiguousarray(np.concatenate([m2, co, rgb, dep[:, None]], 1), np.float32)
+
+    def backward_acc(self, dL_dcolor, dL_ddepth, shift=None):
+        """The render-stage sums of ro_backward in float64, [P][12] = {colour r,g,b, depth, mean2D x,y, conic xx,xy,yy,
+        cov_zx, cov_yz, opacity}.  shift=(g, x0, y0) plants a one-column offset for Gaussian g in the 8x4 sub-tile at
+        (x0, y0)."""
+        P = self.P
+        gc, gd = _f32(dL_dcolor), _f32(dL_ddepth)
+        z = lambda *s: np.zeros(s, np.float32)
+        outs = [z(P, 3), z(P, 3), z(P, 1), z(P, 3), z(P, 6), z(P, max(self.args.M, 1), 3), z(P, 3), z(P, 4)]
+        acc = np.zeros((P, 12), np.float64)
+        sh = None if shift is None else np.asarray(shift, np.int32)
+        _lib.ro_backward_ex(C.byref(self.args), self.st, self.radii.ctypes.data, gc.ctypes.data, gd.ctypes.data,
+                            *[o.ctypes.data for o in outs], acc.ctypes.data, _p(sh))
+        return acc
+
+    def free(self):
+        if self.st:
+            _lib.ro_free(self.st)
+            self.st = None
+
+
+MOMENTS = ["t", "t dx", "t dy", "t dx2", "t dxdy", "t dy2", "v", "v dx", "v dy", "w r", "w g", "w b"]
+RENDER_GRADS = ["colour r", "colour g", "colour b", "depth", "mean2D x", "mean2D y", "conic xx", "conic xy", "conic yy",
+                "cov_zx", "cov_yz", "opacity"]
+
+
+def moment_reference(splats, point_list, ranges, n_contrib, W, H, bg, dL_dcolor, dL_ddepth):
+    """Float64 replay of the render backward from a saved forward state, with a per-Gaussian error bound
+    (ro_moment_reference in raster_oracle.c).  Returns an object with mom, mom_bound, grad, grad_bound ([P][12] float64),
+    n_pairs, S_g, deepest, n_amb ([P] int) and pairs, ambiguous, max_contrib (ints)."""
+    global _lib
+    if _lib is None:
+        _lib = _load()
+    sp = _f32(splats).reshape(-1, 12)
+    P = sp.shape[0]
+    pl = np.ascontiguousarray(point_list, np.uint32).reshape(-1)
+    rg = np.ascontiguousarray(ranges, np.uint32).reshape(-1, 2)
+    nc = np.ascontiguousarray(n_contrib, np.uint32).reshape(-1)
+    assert nc.size == W * H and rg.shape[0] == ((W + 15) // 16) * ((H + 15) // 16)
+    gc, gd, bgc = _f32(dL_dcolor).reshape(3, H * W), _f32(dL_ddepth).reshape(H * W), _f32(bg).reshape(3)
+    r = Result()
+    r.mom, r.mom_bound, r.grad, r.grad_bound = (np.zeros((P, 12), np.float64) for _ in range(4))
+    diag = np.zeros((P, 4), np.int32)
+    tot = np.zeros(3, np.int64)
+    _lib.ro_moment_reference(P, W, H, sp.ctypes.data, pl.ctypes.data if pl.size else None, rg.ctypes.data,
+                             nc.ctypes.data, bgc.ctypes.data, gc.ctypes.data, gd.ctypes.data, r.mom.ctypes.data,
+                             r.mom_bound.ctypes.data, r.grad.ctypes.data, r.grad_bound.ctypes.data, diag.ctypes.data,
+                             tot.ctypes.data)
+    r.n_pairs, r.S_g, r.deepest, r.n_amb = (diag[:, k].copy() for k in range(4))
+    r.pairs, r.ambiguous, r.max_contrib = (int(v) for v in tot)
     return r
