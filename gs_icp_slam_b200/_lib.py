@@ -79,6 +79,7 @@ _sig("gsicp_prof_read", i32, [i32, f64p, C.POINTER(C.c_long)])
 _sig("gsicp_raster_forward", i32, [C.POINTER(RasterArgs), vp, vp, vp, vp, ALLOC_FN, ALLOC_FN, ALLOC_FN, vp, vp])
 _sig("gsicp_raster_backward_work_bytes", C.c_size_t, [i32])
 _sig("gsicp_raster_set_allreduce", i32, [ALLREDUCE_F32_FN, vp])
+_sig("gsicp_raster_set_deterministic", i32, [i32])
 _sig("gsicp_raster_backward", i32, [C.POINTER(RasterArgs), i32, vp, vp, vp, vp, vp, vp] + [vp] * 8 + [vp, vp])
 _sig("gsicp_raster_export_binning", i32, [C.POINTER(RasterArgs), i32, vp, vp, vp, vp, vp])
 _sig("gsicp_mark_visible", i32, [i32, vp, vp, vp, vp, vp])
@@ -88,6 +89,8 @@ _sig("gsicp_test_preload_kernels", i32, [])
 _sig("gsicp_test_grid_meta", i32, [vp, i32, C.POINTER(C.c_float), C.POINTER(C.c_int)])
 _sig("gsicp_test_raster_state", i32, [C.POINTER(RasterArgs), i32, i32, vp, vp, vp, vp, vp, vp])
 _sig("gsicp_test_set_moment_tap", None, [vp])
+_sig("gsicp_test_set_bwd_tile_order", None, [i32, C.c_uint])
+_sig("gsicp_test_last_bwd_mode", i32, [])
 _sig("gsicp_dist2", i32, [i32, vp, vp, vp])
 
 _sig("gsicp_gicp_create", vp, [])

@@ -19,8 +19,11 @@
 // per-Gaussian backward: computeCov2D backward and the preprocess backward are one kernel (the
 // intermediate dL_dcov3D / dL_dmeans never round-trip through HBM between two launches).
 #include <cub/cub.cuh>
+#include <algorithm>
 #include <cstdlib>
 #include <mutex>
+#include <random>
+#include <vector>
 #include "host_common.h"
 #include "raster_common.cuh"
 #include "comm.cuh"
@@ -83,14 +86,58 @@ __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__flo
 // 2-CTA-per-SM build (262-276 us): the kernel wants resident warps, not more ILP per warp.
 // kStage / kMinBlocks: (256, 3) = 80 registers, 58 KB of shared memory, 3 CTAs per SM (default);
 // (128, 4) = 64 registers, 46 KB, 4 CTAs per SM (experiment: GSICP_BWD_VARIANT=1).
-template <bool kCull, int kStage = kTilePixels, int kMinBlocks = 3>
+//
+// Deterministic mode (gsicp_raster_set_deterministic): the per-(sub-tile, survivor group) contributions c are already a
+// function of the list, the cull masks and the pixels only; what varies from run to run is the order of the float adds.
+// There the kernel runs twice with integer atomics only, which are associative:
+//   kDetExp (pass A): atomicMax of the biased fp32 exponent field e of every contribution, per Gaussian and moment, and
+//                     atomicAdd of the Gaussian's contribution count n.  Then |c| < 2^(E - 126) for E = max e, and E = 255
+//                     iff some contribution is not finite.
+//   kDetSum (pass B): acc += llrint(c 2^(S + 126 - E)) in int64, S = 62 - ceil(log2 n).  The scaling is exact (fp32 times
+//                     a power of two, in double); every term is at most 2^S in magnitude, so no partial sum, in any order,
+//                     leaves (-2^62, 2^62).  The rounding error is at most n/2 2^(E - 126 - S).  Where E = 255 the finite
+//                     terms are dropped and acc collects flags instead: 1 = +inf, 2 = -inf, 4 = NaN.
+// det_convert_kernel then writes float(double(acc) 2^(E - 126 - S)) into the float moment rows.
+enum { kDetOff = 0, kDetExp = 1, kDetSum = 2 };
+struct DetRow {         // per-Gaussian scratch of the deterministic mode (152 B): zero between backwards
+  long long acc[kG];    // fixed-point sums (pass B), or non-finite flags
+  int E[kG];            // largest biased exponent field of the contributions (pass A)
+  uint32_t n;           // contributions (pass A)
+  uint32_t pad;
+};
+static_assert(sizeof(DetRow) == 152, "DetRow layout");
+
+// 2^k as a double, k in [-1022, 1023]
+__device__ __forceinline__ double exp2i(int k) { return __longlong_as_double((long long)(k + 1023) << 52); }
+__device__ __forceinline__ int det_scale(uint32_t n) { return 62 - (n > 1 ? 32 - __clz(n - 1) : 0); }  // S
+
+template <int kDet>
+__device__ __forceinline__ void det_contribute(DetRow* __restrict__ row, int k, float c) {
+  if (c == 0.f) return;  // adds nothing in either pass
+  const int e = (int)((__float_as_uint(c) >> 23) & 0xffu);
+  if (kDet == kDetExp) {
+    atomicMax(&row->E[k], e);
+  } else {
+    const int E = row->E[k];
+    unsigned long long* acc = reinterpret_cast<unsigned long long*>(&row->acc[k]);
+    if (E == 255) {
+      if (e == 255) atomicOr(acc, c != c ? 4ull : c > 0.f ? 1ull : 2ull);
+      return;
+    }
+    const double v = (double)c * exp2i(det_scale(row->n) + 126 - E);
+    atomicAdd(acc, (unsigned long long)__double2ll_rn(v));
+  }
+}
+
+template <bool kCull, int kStage = kTilePixels, int kMinBlocks = 3, int kDet = kDetOff>
 __global__ void __launch_bounds__(kTilePixels, kMinBlocks)
 render_backward_kernel(const uint32_t* __restrict__ tile_order, const uint2* __restrict__ ranges,
                        const uint32_t* __restrict__ point_list, int W, int H,
                        int tiles_x, const float* __restrict__ bg, const Splat* __restrict__ splats,
                        const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
                        const float* __restrict__ dL_dpix_color, const float* __restrict__ dL_dpix_depth,
-                       float* __restrict__ moments, const uint32_t* __restrict__ hit_in, int shard_count, int shard_index) {
+                       float* __restrict__ moments, const uint32_t* __restrict__ hit_in, int shard_count, int shard_index,
+                       DetRow* __restrict__ det) {
   const int tile = (int)tile_order[blockIdx.x];
   if (shard_count > 1 && (tile % shard_count) != shard_index) return;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -222,9 +269,16 @@ render_backward_kernel(const uint32_t* __restrict__ tile_order, const uint2* __r
       const float gt = ((r_1 | r_2) ? -own_t : own_t) + (p * q) * S0 - cross;
       const float gw = (r_1 | r_2) ? p * V0 - own_w : own_w;
       if (g8 < 6 && n < cnt) {
-        float* dst = moments + (size_t)gid * kG;
-        atomicAdd(dst + g8, gt);
-        atomicAdd(dst + 6 + g8, gw);
+        if (kDet == kDetOff) {
+          float* dst = moments + (size_t)gid * kG;
+          atomicAdd(dst + g8, gt);
+          atomicAdd(dst + 6 + g8, gw);
+        } else {
+          DetRow* row = det + gid;
+          if (kDet == kDetExp && g8 == 0) atomicAdd(&row->n, 1u);
+          det_contribute<kDet>(row, g8, gt);
+          det_contribute<kDet>(row, 6 + g8, gw);
+        }
       }
     }
     cnt = 0;
@@ -732,6 +786,43 @@ __global__ void moments_gather_slices_kernel(CommView c, int P, int slice, const
   dst[0] = __ldcv(src); dst[1] = __ldcv(src + 1); dst[2] = __ldcv(src + 2);
 }
 
+// Deterministic mode, after pass B: the fixed-point sums into the float moment rows (which are zero on entry, like the
+// accumulator of the default mode), then the scratch rows back to zero.  Every row the two passes touched belongs to a
+// visible Gaussian, so all of them are cleaned.
+__global__ void det_convert_kernel(int P, const int32_t* __restrict__ radii, DetRow* __restrict__ det,
+                                   float* __restrict__ moments) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P || !(radii[i] > 0)) return;
+  DetRow* row = det + i;
+  const uint32_t n = row->n;
+  if (n == 0) return;  // not blended anywhere: the float row stays zero and so does the scratch row
+  const int S = det_scale(n);
+  float out[kG];
+#pragma unroll
+  for (int k = 0; k < kG; k++) {
+    const long long a = row->acc[k];
+    const int E = row->E[k];
+    if (E == 255)
+      out[k] = ((a & 4) || (a & 3) == 3) ? __int_as_float(0x7fc00000) : __int_as_float((a & 1) ? 0x7f800000 : 0xff800000);
+    else
+      out[k] = (float)((double)a * exp2i(E - 126 - S));
+  }
+  float4* m = reinterpret_cast<float4*>(moments) + 3 * (size_t)i;
+  m[0] = make_float4(out[0], out[1], out[2], out[3]);
+  m[1] = make_float4(out[4], out[5], out[6], out[7]);
+  m[2] = make_float4(out[8], out[9], out[10], out[11]);
+  long long* z = reinterpret_cast<long long*>(row);
+#pragma unroll
+  for (int k = 0; k < (int)(sizeof(DetRow) / 8); k++) z[k] = 0;
+}
+
+// Test hook: render_backward's CTAs visit out[b] = tile_order[perm[b]] instead of tile_order[b].
+__global__ void permute_tile_order_kernel(int tiles, const uint32_t* __restrict__ perm, const uint32_t* __restrict__ tile_order,
+                                          uint32_t* __restrict__ out) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < tiles) out[b] = tile_order[perm[b]];
+}
+
 gsicp_comm* g_raster_comm = nullptr;  // set by gsicp_raster_set_comm; also read by the forward pass (raster_forward.cu)
 
 // Where this rank's render moments accumulate: the exchange segment in a sharded run, else the geometry buffer.
@@ -817,9 +908,104 @@ static int ensure_bwd_smem_attr() {
   GSICP_CUDA(cudaFuncSetAttribute(render_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmem)));
   GSICP_CUDA(cudaFuncSetAttribute((render_backward_kernel<true, 128, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)sizeof(BwdSmemT<128>)));
+  for (int pass : {kDetExp, kDetSum}) {
+    const bool a = pass == kDetExp;
+    GSICP_CUDA(cudaFuncSetAttribute(a ? render_backward_kernel<true, kTilePixels, 3, kDetExp> : render_backward_kernel<true, kTilePixels, 3, kDetSum>,
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmem)));
+    GSICP_CUDA(cudaFuncSetAttribute(a ? render_backward_kernel<false, kTilePixels, 3, kDetExp> : render_backward_kernel<false, kTilePixels, 3, kDetSum>,
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmem)));
+    GSICP_CUDA(cudaFuncSetAttribute(a ? render_backward_kernel<true, 128, 4, kDetExp> : render_backward_kernel<true, 128, 4, kDetSum>,
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmemT<128>)));
+  }
   done[dev] = true;
   return GSICP_OK;
 }
+
+// One launch of render_backward_kernel in the configuration the test switches select (sub-tile cull off; staging variant).
+struct RenderBwdLaunch {
+  const uint32_t* tile_order; const uint2* ranges; const uint32_t* point_list; int W, H, tiles_x, tiles; const float* bg;
+  const Splat* splats; const float* final_T; const uint32_t* n_contrib; const float* dpix_color; const float* dpix_depth;
+  float* moments; const uint32_t* hit; int shard_count, shard_index; cudaStream_t stream;
+};
+template <int kDet>
+static void launch_render_backward(const RenderBwdLaunch& l, DetRow* det) {
+  if (!g_render_cull) {  // test hook: no sub-tile culling
+    GSICP_LAUNCH((render_backward_kernel<false, kTilePixels, 3, kDet>), l.tiles, kTilePixels, sizeof(BwdSmem), l.stream, l.tile_order,
+                 l.ranges, l.point_list, l.W, l.H, l.tiles_x, l.bg, l.splats, l.final_T, l.n_contrib, l.dpix_color, l.dpix_depth,
+                 l.moments, l.hit, l.shard_count, l.shard_index, det);
+  } else if (g_bwd_variant == 1) {
+    GSICP_LAUNCH((render_backward_kernel<true, 128, 4, kDet>), l.tiles, kTilePixels, sizeof(BwdSmemT<128>), l.stream, l.tile_order,
+                 l.ranges, l.point_list, l.W, l.H, l.tiles_x, l.bg, l.splats, l.final_T, l.n_contrib, l.dpix_color, l.dpix_depth,
+                 l.moments, l.hit, l.shard_count, l.shard_index, det);
+  } else {
+    GSICP_LAUNCH((render_backward_kernel<true, kTilePixels, 3, kDet>), l.tiles, kTilePixels, sizeof(BwdSmem), l.stream, l.tile_order,
+                 l.ranges, l.point_list, l.W, l.H, l.tiles_x, l.bg, l.splats, l.final_T, l.n_contrib, l.dpix_color, l.dpix_depth,
+                 l.moments, l.hit, l.shard_count, l.shard_index, det);
+  }
+}
+
+// Scratch of the deterministic mode, one set per device, grow-only, zero between backwards (zeroed once when it grows,
+// re-zeroed row by row by det_convert_kernel).  Backwards on different streams of one device are ordered through `done`.
+constexpr int kDetMaxDevices = 64;
+struct DetScratch {
+  std::mutex mu;
+  Scratch rows;               // DetRow[P]
+  cudaEvent_t done = nullptr;  // recorded after the last deterministic backward's det_convert_kernel
+};
+static DetScratch g_det_dev[kDetMaxDevices];
+static std::atomic<int> g_deterministic{0};
+static std::atomic<int> g_last_bwd_mode{-1};  // test hook: 0 = float atomics, 1 = deterministic
+
+// Passes A and B and the conversion into l.moments.
+static int render_backward_deterministic(const RenderBwdLaunch& l, int P, const int32_t* d_radii) {
+  int dev = 0;
+  GSICP_CUDA(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= kDetMaxDevices) {
+    set_error("gsicp_raster_backward: device index %d out of range", dev);
+    return GSICP_EINVAL;
+  }
+  DetScratch& d = g_det_dev[dev];
+  std::lock_guard<std::mutex> lock(d.mu);
+  if (!d.done) GSICP_CUDA(cudaEventCreateWithFlags(&d.done, cudaEventDisableTiming));
+  else GSICP_CUDA(cudaStreamWaitEvent(l.stream, d.done, 0));
+  const size_t cap = d.rows.cap;
+  if (int e = d.rows.ensure((size_t)P * sizeof(DetRow))) return e;
+  if (d.rows.cap != cap) GSICP_CUDA(cudaMemsetAsync(d.rows.ptr, 0, d.rows.cap, l.stream));
+  DetRow* det = d.rows.as<DetRow>();
+  launch_render_backward<kDetExp>(l, det);
+  launch_render_backward<kDetSum>(l, det);
+  GSICP_LAUNCH(det_convert_kernel, (P + 255) / 256, 256, 0, l.stream, P, d_radii, det, l.moments);
+  GSICP_CUDA(cudaEventRecord(d.done, l.stream));
+  return GSICP_OK;
+}
+
+// Test hook: 0 = the forward's tile order, 1 = reversed, 2 = a shuffle seeded by `seed`.
+static int g_tile_perm = 0;
+static unsigned g_tile_perm_seed = 0;
+static Scratch g_tile_perm_buf;
+
+static int permuted_tile_order(int tiles, const uint32_t* tile_order, cudaStream_t stream, const uint32_t** out) {
+  std::vector<uint32_t> perm(tiles);
+  for (int b = 0; b < tiles; b++) perm[b] = g_tile_perm == 1 ? (uint32_t)(tiles - 1 - b) : (uint32_t)b;
+  if (g_tile_perm == 2) std::shuffle(perm.begin(), perm.end(), std::mt19937(g_tile_perm_seed));
+  if (int e = g_tile_perm_buf.ensure((size_t)tiles * 8)) return e;
+  uint32_t* d_perm = g_tile_perm_buf.as<uint32_t>();
+  GSICP_CUDA(cudaMemcpyAsync(d_perm, perm.data(), (size_t)tiles * 4, cudaMemcpyHostToDevice, stream));
+  GSICP_CUDA(cudaStreamSynchronize(stream));  // `perm` is pageable host memory and goes out of scope
+  GSICP_LAUNCH(permute_tile_order_kernel, (tiles + 255) / 256, 256, 0, stream, tiles, d_perm, tile_order, d_perm + tiles);
+  *out = d_perm + tiles;
+  return GSICP_OK;
+}
+
+extern "C" int gsicp_raster_set_deterministic(int on) {
+  g_deterministic.store(on ? 1 : 0);
+  return GSICP_OK;
+}
+extern "C" void gsicp_test_set_bwd_tile_order(int mode, unsigned seed) {
+  g_tile_perm = mode;
+  g_tile_perm_seed = seed;
+}
+extern "C" int gsicp_test_last_bwd_mode(void) { return g_last_bwd_mode.load(); }
 
 extern "C" int gsicp_raster_set_allreduce(gsicp_allreduce_f32_fn fn, void* user) {
   std::lock_guard<std::mutex> lock(g_bwd.mu);
@@ -905,21 +1091,21 @@ extern "C" int gsicp_raster_backward(const gsicp_raster_args* args, int num_rend
   }
   float* work = raster_moment_accumulator(args, geom.moments);  // [P][12]
 
+  const bool deterministic = g_deterministic.load() != 0;
+  g_last_bwd_mode.store(deterministic ? 1 : 0);
   if (num_rendered > 0) {
     if (int e = ensure_bwd_smem_attr()) return e;
+    const uint32_t* tile_order = img.tile_order;
+    if (g_tile_perm)
+      if (int e = permuted_tile_order(tiles, img.tile_order, stream, &tile_order)) return e;
+    const RenderBwdLaunch l = {tile_order, img.ranges, bin.point_list, W, H, tiles_x, tiles, args->d_background, geom.splats,
+                               img.final_T, img.n_contrib, d_dL_dout_color, d_dL_dout_depth, work, bin.hit, shard_count,
+                               shard_index, stream};
     ProfScope ps(kProfRenderBwd, stream);
-    if (!g_render_cull) {  // test hook: no sub-tile culling
-      GSICP_LAUNCH(render_backward_kernel<false>, tiles, kTilePixels, sizeof(BwdSmem), stream, img.tile_order, img.ranges, bin.point_list,
-                   W, H, tiles_x, args->d_background, geom.splats, img.final_T, img.n_contrib, d_dL_dout_color, d_dL_dout_depth,
-                   work, bin.hit, shard_count, shard_index);
-    } else if (g_bwd_variant == 1) {
-      GSICP_LAUNCH((render_backward_kernel<true, 128, 4>), tiles, kTilePixels, sizeof(BwdSmemT<128>), stream, img.tile_order, img.ranges,
-                   bin.point_list, W, H, tiles_x, args->d_background, geom.splats, img.final_T, img.n_contrib, d_dL_dout_color,
-                   d_dL_dout_depth, work, bin.hit, shard_count, shard_index);
+    if (deterministic) {
+      if (int e = render_backward_deterministic(l, P, d_radii)) return e;
     } else {
-      GSICP_LAUNCH(render_backward_kernel<true>, tiles, kTilePixels, sizeof(BwdSmem), stream, img.tile_order, img.ranges, bin.point_list,
-                   W, H, tiles_x, args->d_background, geom.splats, img.final_T, img.n_contrib, d_dL_dout_color, d_dL_dout_depth,
-                   work, bin.hit, shard_count, shard_index);
+      launch_render_backward<kDetOff>(l, nullptr);
     }
     if (args->debug) GSICP_CUDA(cudaStreamSynchronize(stream));
   }

@@ -26,6 +26,8 @@ def set_tile_shard(count, index):
     _tile_shard = (int(count), int(index))
 
 
+_deterministic = False  # the library's mode (gsicp_raster_set_deterministic), as last set from here
+
 _allreduce_cb = None  # keeps the ctypes thunk alive
 
 
@@ -210,10 +212,16 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     """_C.rasterize_gaussians_backward (rasterize_points.cu:123-206).
 
     Returns (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations)."""
+    global _deterministic
     dev = means3D.device
     P = means3D.size(0)
     H, W = dL_dout_color.size(1), dL_dout_color.size(2)
     M = sh.size(1) if sh.numel() != 0 else 0
+    # torch.use_deterministic_algorithms(True) selects the library's bit-reproducible render backward
+    det = torch.are_deterministic_algorithms_enabled()
+    if det != _deterministic:
+        check(lib.gsicp_raster_set_deterministic(int(det)), "gsicp_raster_set_deterministic")
+        _deterministic = det
     with _on_device(dev):
         # One UNINITIALISED slab for the eight gradient tensors: the per-Gaussian backward kernel writes every element
         # (zeros for Gaussians outside the view), so no fill launch precedes it.  The kernels are launched from raw offsets

@@ -107,6 +107,11 @@ size_t gsicp_raster_backward_work_bytes(int P);
  * the render-backward and the per-Gaussian-backward kernels; every rank then returns the FULL parameter gradients. */
 typedef int (*gsicp_allreduce_f32_fn)(void* user, float* d_buf, size_t count, void* stream);
 int gsicp_raster_set_allreduce(gsicp_allreduce_f32_fn fn, void* user);
+/* Process-wide (default 0).  With 1, gsicp_raster_backward sums each Gaussian's render moments in fixed point with integer
+ * atomics instead of float atomics: the gradients are bit-identical for the same forward state and dL/dpix, whatever the
+ * CTA schedule or the tile launch order.  It runs the render backward twice (exponents, then sums); it needs
+ * 152 B of library-internal scratch per Gaussian on each device (grow-only) and still no caller work buffer. */
+int gsicp_raster_set_deterministic(int on);
 int gsicp_raster_backward(const gsicp_raster_args* args, int num_rendered,
                           const int32_t* d_radii,
                           const void* d_geom, const void* d_binning, const void* d_image,
