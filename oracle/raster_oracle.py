@@ -116,7 +116,7 @@ class State:
     tile ranges and per-pixel n_contrib / final_T the backward reads.  `final_T` is a writable view of the state itself.
     Call free() when done."""
 
-    def __init__(self, scene, cam, H, W, bg, sh_degree=0):
+    def __init__(self, scene, cam, H, W, bg, sh_degree=0, scale_modifier=1.0):
         global _lib
         if _lib is None:
             _lib = _load()
@@ -126,7 +126,8 @@ class State:
         means, shs, opac, scales, rots, view, proj, campos, bgc = self.keep
         P = self.P = means.shape[0]
         self.H, self.W, self.bg = H, W, bgc
-        self.args = _Args(P, sh_degree, shs.shape[1], W, H, cam["tanfovx"], cam["tanfovy"], 1.0, _p(bgc), _p(means),
+        self.args = _Args(P, sh_degree, shs.shape[1], W, H, cam["tanfovx"], cam["tanfovy"], scale_modifier, _p(bgc),
+                          _p(means),
                           _p(shs), None, _p(opac), _p(scales), _p(rots), None, _p(view), _p(proj), _p(campos))
         self.color = np.zeros((3, H, W), np.float32)
         self.depth = np.zeros((1, H, W), np.float32)
@@ -147,10 +148,10 @@ class State:
         # the GPU's record layout: {px, py, conic xx, xy, yy, opacity, cov_zx, cov_yz, r, g, b, depth}
         self.splats = np.ascontiguousarray(np.concatenate([m2, co, rgb, dep[:, None]], 1), np.float32)
 
-    def backward_acc(self, dL_dcolor, dL_ddepth, shift=None):
+    def backward_acc(self, dL_dcolor, dL_ddepth, shift=None, with_outputs=False):
         """The render-stage sums of ro_backward in float64, [P][12] = {colour r,g,b, depth, mean2D x,y, conic xx,xy,yy,
         cov_zx, cov_yz, opacity}.  shift=(g, x0, y0) plants a one-column offset for Gaussian g in the 8x4 sub-tile at
-        (x0, y0)."""
+        (x0, y0).  with_outputs: (acc, the eight float32 gradient arrays of ro_backward computed from float32(acc))."""
         P = self.P
         gc, gd = _f32(dL_dcolor), _f32(dL_ddepth)
         z = lambda *s: np.zeros(s, np.float32)
@@ -159,7 +160,7 @@ class State:
         sh = None if shift is None else np.asarray(shift, np.int32)
         _lib.ro_backward_ex(C.byref(self.args), self.st, self.radii.ctypes.data, gc.ctypes.data, gd.ctypes.data,
                             *[o.ctypes.data for o in outs], acc.ctypes.data, _p(sh))
-        return acc
+        return (acc, outs) if with_outputs else acc
 
     def free(self):
         if self.st:
