@@ -21,6 +21,27 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
+
+int wait_published(const volatile unsigned long long* word, unsigned long long seq, cudaStream_t stream, const char* what) {
+  long spins = 0;
+  while (*word != seq) {
+#if defined(__x86_64__)
+    __builtin_ia32_pause();
+#endif
+    if ((++spins & 0xfffff) == 0) {
+      const cudaError_t q = cudaStreamQuery(stream);
+      if (q != cudaSuccess && q != cudaErrorNotReady) {
+        set_error("%s failed: %s", what, cudaGetErrorString(q));
+        return GSICP_ECUDA;
+      }
+      if (q == cudaSuccess && *word != seq) {
+        set_error("%s was not published", what);
+        return GSICP_ECUDA;
+      }
+    }
+  }
+  return GSICP_OK;
+}
 }  // namespace gsicp
 
 namespace gsicp {

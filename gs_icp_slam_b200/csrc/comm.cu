@@ -35,13 +35,13 @@ int comm_preload_kernels() {
 
 int comm_stream_barrier(gsicp_comm* c, cudaStream_t stream) {
   if (!c || !c->connected || c->world <= 1) return GSICP_OK;
-  if (c->h_status && *(volatile int*)c->h_status) {
+  if (c->status.h && *(volatile int*)c->status.h) {
     set_error("exchange group (rank %d of %d): an earlier barrier ran out of its poll budget - a peer did not arrive; results since "
               "then are not valid", c->rank, c->world);
     return GSICP_ECUDA;
   }
   const unsigned long long seq = ++c->bar_seq;
-  GSICP_LAUNCH(comm_barrier_kernel, 1, 32, 0, stream, c->view(), seq, c->d_status);
+  GSICP_LAUNCH(comm_barrier_kernel, 1, 32, 0, stream, c->view(), seq, c->status.d);
   GSICP_CUDA(cudaGetLastError());
   return GSICP_OK;
 }
@@ -56,7 +56,7 @@ extern "C" int gsicp_comm_alloc(size_t heap_bytes, gsicp_comm** out, void* handl
   gsicp_comm* c = new gsicp_comm();
   auto fail = [&](int code, const char* what, cudaError_t e) {
     set_error("gsicp_comm_alloc: %s failed: %s", what, cudaGetErrorString(e));
-    if (c->h_status) cudaFreeHost(c->h_status);
+    c->status.free();
     if (c->local) cudaFree(c->local);
     delete c;
     return code;
@@ -66,9 +66,7 @@ extern "C" int gsicp_comm_alloc(size_t heap_bytes, gsicp_comm** out, void* handl
   c->bytes = kCommHeapOff + ((heap_bytes + 255) & ~size_t(255));
   if ((e = cudaMalloc((void**)&c->local, c->bytes)) != cudaSuccess) return fail(GSICP_ENOMEM, "cudaMalloc", e);
   if ((e = cudaMemset(c->local, 0, c->bytes)) != cudaSuccess) return fail(GSICP_ECUDA, "cudaMemset", e);
-  if ((e = cudaHostAlloc((void**)&c->h_status, 64, cudaHostAllocMapped)) != cudaSuccess) return fail(GSICP_ENOMEM, "cudaHostAlloc", e);
-  *c->h_status = 0;
-  if ((e = cudaHostGetDevicePointer((void**)&c->d_status, c->h_status, 0)) != cudaSuccess) return fail(GSICP_ECUDA, "cudaHostGetDevicePointer", e);
+  if ((e = c->status.alloc(16)) != cudaSuccess) return fail(GSICP_ENOMEM, "mapped status allocation", e);
   cudaIpcMemHandle_t h;
   if ((e = cudaIpcGetMemHandle(&h, c->local)) != cudaSuccess) return fail(GSICP_ECUDA, "cudaIpcGetMemHandle", e);
   std::memcpy(handle64, &h, 64);
@@ -123,7 +121,7 @@ extern "C" void gsicp_comm_destroy(gsicp_comm* c) {
   for (int r = 0; r < c->world; r++)
     if (!c->local_only && r != c->rank && c->peer[r]) cudaIpcCloseMemHandle(c->peer[r]);
   if (c->local) cudaFree(c->local);
-  if (c->h_status) cudaFreeHost(c->h_status);
+  c->status.free();
   delete c;
 }
 

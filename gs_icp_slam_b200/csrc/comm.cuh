@@ -16,6 +16,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "host_common.h"
 
 namespace gsicp {
 
@@ -113,8 +114,7 @@ struct gsicp_comm {
   unsigned long long bar_seq = 0;  // stream-barrier sequence (host-side counter; identical call order on every rank)
   unsigned long long lm_seq = 0;   // last LM exchange sequence number handed out (host-side, identical on every rank)
   bool lm_resync = false;          // the last launch consumed a data-dependent number of exchanges: re-align with a barrier
-  int* h_status = nullptr;         // mapped pinned word: a barrier kernel sets it when its poll budget ran out (a peer is gone)
-  int* d_status = nullptr;         // device alias of h_status
+  gsicp::Mapped<int> status;       // status.h[0]: a barrier kernel sets it when its poll budget ran out (a peer is gone)
   gsicp::CommView view() const {
     gsicp::CommView v;
     v.world = world;

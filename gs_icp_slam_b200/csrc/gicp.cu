@@ -832,9 +832,7 @@ align_lm_kernel(LmArgs a) {
     r->n_err = n_err;
     mark();
     r->n_marks = n_marks;
-    __threadfence_system();
-    *(volatile unsigned long long*)&r->seq = a.seq;
-    __threadfence_system();
+    publish_seq(&r->seq, a.seq);
   }
 }
 
@@ -902,8 +900,7 @@ struct gsicp_gicp {
   Scratch corr, sqd, mahal, partial, red_out, counter, staging_dev, nn_id, nn_d2;
   int corr_n = 0;
   double* h_red = nullptr;     // pinned [28]
-  unsigned long long* h_map = nullptr;  // mapped pinned: [0..27] sums (as double), [28] sequence word
-  unsigned long long* d_map = nullptr;  // device alias of h_map
+  Mapped<unsigned long long> map;  // [0..27] sums (as double), [28] sequence word
   unsigned long long seq = 0;
   void* h_stage = nullptr;     // pinned staging for H2D conversions
   size_t h_stage_cap = 0;
@@ -914,8 +911,7 @@ struct gsicp_gicp {
   void* reduce_user = nullptr;
   bool host_lm = false;          // GSICP_HOST_LM=1: host-driven LM loop (one launch + one spin-wait per phase)
   Scratch lm_partL, lm_partE, lm_barrier;
-  LmResult* h_lm = nullptr;      // mapped pinned result block of align_lm_kernel
-  LmResult* d_lm = nullptr;
+  Mapped<LmResult> lm;           // result block of align_lm_kernel
   int lm_max_blocks = 0;         // co-resident blocks of align_lm_kernel on this device
   bool timing = false;
   double t_cov = 0, t_lin = 0, t_err = 0;
@@ -1237,33 +1233,21 @@ int ensure_lin_buffers(gsicp_gicp* h) {
     GSICP_CUDA(cudaMemsetAsync(h->counter.ptr, 0, sizeof(unsigned int), h->stream));
   }
   if (!h->h_red) GSICP_CUDA(cudaMallocHost(&h->h_red, kRed * sizeof(double)));
-  if (!h->h_map) {
-    GSICP_CUDA(cudaHostAlloc((void**)&h->h_map, 32 * sizeof(unsigned long long), cudaHostAllocMapped));
-    std::memset(h->h_map, 0, 32 * sizeof(unsigned long long));
-    GSICP_CUDA(cudaHostGetDevicePointer((void**)&h->d_map, h->h_map, 0));
-  }
+  GSICP_CUDA(h->map.alloc(32));
   return GSICP_OK;
 }
 
-// Spin until the kernel's last block has published sequence number `seq` into mapped host memory.
-int wait_published(gsicp_gicp* h, unsigned long long seq) {
-  volatile unsigned long long* p = h->h_map + 28;
-  long spins = 0;
-  while (*p != seq) {
-#if defined(__x86_64__)
-    __builtin_ia32_pause();
-#endif
-    if ((++spins & 0xfffff) == 0) {  // every ~1M spins make sure the kernel has not failed
-      const cudaError_t q = cudaStreamQuery(h->stream);
-      if (q != cudaSuccess && q != cudaErrorNotReady) {
-        set_error("kernel failed: %s", cudaGetErrorString(q));
-        return GSICP_ECUDA;
-      }
-      if (q == cudaSuccess && *p != seq) {
-        set_error("reduction result was not published");
-        return GSICP_ECUDA;
-      }
-    }
+// The first n sums of a linearize / error launch into h_red: read from the mailbox its last block published into
+// (direct), or copied from red_out with a stream synchronise (timing runs, and the all-reduce callback of sharded runs).
+int read_sums(gsicp_gicp* h, bool direct, unsigned long long seq, int n, StageTimer& tm) {
+  if (direct) {
+    GSICP_CUDA(cudaGetLastError());
+    if (int e = wait_published(&h->map.h[28], seq, h->stream, "reduction result")) return e;
+    std::memcpy(h->h_red, h->map.h, n * sizeof(double));
+  } else {
+    GSICP_CUDA(cudaMemcpyAsync(h->h_red, h->red_out.ptr, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    tm.stop();
+    GSICP_CUDA(cudaStreamSynchronize(h->stream));
   }
   return GSICP_OK;
 }
@@ -1391,8 +1375,8 @@ int run_linearize(gsicp_gicp* h, const Iso& x, double H[6][6], double b[6], doub
   a.partial = h->partial.as<double>(); a.out = h->red_out.as<double>(); a.counter = h->counter.as<unsigned int>();
   const bool xchg = h->shard_count > 1 && h->comm;  // in-kernel exchange: the published sums are already global
   const bool direct = (h->shard_count <= 1 || xchg) && !h->timing;  // publish straight into mapped host memory
-  a.host_out = direct ? (double*)h->d_map : nullptr;
-  a.host_seq = direct ? (volatile unsigned long long*)(h->d_map + 28) : nullptr;
+  a.host_out = direct ? (double*)h->map.d : nullptr;
+  a.host_seq = direct ? &h->map.d[28] : nullptr;
   a.seq = ++h->seq;
   a.comm = CommView();
   a.xseq = 0;
@@ -1424,15 +1408,7 @@ int run_linearize(gsicp_gicp* h, const Iso& x, double H[6][6], double b[6], doub
       return GSICP_ECUDA;
     }
   }
-  if (direct) {
-    GSICP_CUDA(cudaGetLastError());
-    if (int e = wait_published(h, a.seq)) return e;
-    std::memcpy(h->h_red, h->h_map, kRed * sizeof(double));
-  } else {
-    GSICP_CUDA(cudaMemcpyAsync(h->h_red, h->red_out.ptr, kRed * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    tm.stop();
-    GSICP_CUDA(cudaStreamSynchronize(h->stream));
-  }
+  if (int e = read_sums(h, direct, a.seq, kRed, tm)) return e;
   h->n_lin++;
   if (H && b) {
     int o = 0;
@@ -1460,8 +1436,8 @@ int run_error(gsicp_gicp* h, const Iso& x, double* err) {  // fgi:355-378
   a.partial = h->partial.as<double>(); a.out = h->red_out.as<double>(); a.counter = h->counter.as<unsigned int>();
   const bool xchg = h->shard_count > 1 && h->comm;
   const bool direct = (h->shard_count <= 1 || xchg) && !h->timing;
-  a.host_out = direct ? (double*)h->d_map : nullptr;
-  a.host_seq = direct ? (volatile unsigned long long*)(h->d_map + 28) : nullptr;
+  a.host_out = direct ? (double*)h->map.d : nullptr;
+  a.host_seq = direct ? &h->map.d[28] : nullptr;
   a.seq = ++h->seq;
   a.comm = CommView();
   a.xseq = 0;
@@ -1482,15 +1458,7 @@ int run_error(gsicp_gicp* h, const Iso& x, double* err) {  // fgi:355-378
     const int rc = h->reduce(h->reduce_user, h->red_out.as<double>(), 1, (void*)h->stream);
     if (rc != 0) return GSICP_ECUDA;
   }
-  if (direct) {
-    GSICP_CUDA(cudaGetLastError());
-    if (int e = wait_published(h, a.seq)) return e;
-    h->h_red[0] = *(const double*)h->h_map;
-  } else {
-    GSICP_CUDA(cudaMemcpyAsync(h->h_red, h->red_out.ptr, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    tm.stop();
-    GSICP_CUDA(cudaStreamSynchronize(h->stream));
-  }
+  if (int e = read_sums(h, direct, a.seq, 1, tm)) return e;
   h->n_err++;
   *err = h->h_red[0];
   return GSICP_OK;
@@ -1541,11 +1509,7 @@ int run_align_device(gsicp_gicp* h, Iso& x0) {
     GSICP_CUDA(cudaMemsetAsync(h->sqd.ptr, 0, (size_t)(h->src.n + 1) * 4, h->stream));
     h->corr_n = h->src.n;
   }
-  if (!h->h_lm) {
-    GSICP_CUDA(cudaHostAlloc((void**)&h->h_lm, sizeof(LmResult), cudaHostAllocMapped));
-    std::memset(h->h_lm, 0, sizeof(LmResult));
-    GSICP_CUDA(cudaHostGetDevicePointer((void**)&h->d_lm, h->h_lm, 0));
-  }
+  GSICP_CUDA(h->lm.alloc(1));
   if (h->lm_max_blocks == 0) {
     int dev = 0, sms = 0;
     GSICP_CUDA(cudaGetDevice(&dev));
@@ -1583,7 +1547,7 @@ int run_align_device(gsicp_gicp* h, Iso& x0) {
   a.max_iterations = h->max_iterations; a.lm_max_iterations = h->lm_max_iterations;
   a.rot_eps = h->rot_eps; a.trans_eps = h->trans_eps; a.init_lambda_factor = h->lm_init_lambda_factor;
   a.guess = x0;
-  a.result = h->d_lm;
+  a.result = h->lm.d;
   a.seq = ++h->seq;
   static const int s_marks = [] { const char* e = getenv("GSICP_LM_MARKS"); return e ? atoi(e) : 0; }();
   a.marks = s_marks;
@@ -1592,26 +1556,8 @@ int run_align_device(gsicp_gicp* h, Iso& x0) {
     GSICP_LAUNCH(align_lm_kernel, blocks, kLmBlock, 0, h->stream, a);
   }
   GSICP_CUDA(cudaGetLastError());
-  // spin on the sequence word the kernel publishes into mapped pinned memory
-  volatile unsigned long long* p = &h->h_lm->seq;
-  long spins = 0;
-  while (*p != a.seq) {
-#if defined(__x86_64__)
-    __builtin_ia32_pause();
-#endif
-    if ((++spins & 0xfffff) == 0) {
-      const cudaError_t q = cudaStreamQuery(h->stream);
-      if (q != cudaSuccess && q != cudaErrorNotReady) {
-        set_error("align kernel failed: %s", cudaGetErrorString(q));
-        return GSICP_ECUDA;
-      }
-      if (q == cudaSuccess && *p != a.seq) {
-        set_error("align result was not published");
-        return GSICP_ECUDA;
-      }
-    }
-  }
-  const LmResult r = *h->h_lm;
+  if (int e = wait_published(&h->lm.h->seq, a.seq, h->stream, "align result")) return e;
+  const LmResult r = *h->lm.h;
   if (s_marks && r.n_marks > 1) {
     fprintf(stderr, "[lm marks] total %.1f us:", (double)(r.marks[r.n_marks - 1] - r.marks[0]) * 1e-3);
     for (int i = 1; i < r.n_marks; i++) fprintf(stderr, " %.1f", (double)(r.marks[i] - r.marks[i - 1]) * 1e-3);
@@ -1694,9 +1640,9 @@ void gsicp_gicp_destroy(gsicp_gicp* h) {
   fr(h->corr); fr(h->sqd); fr(h->mahal); fr(h->partial); fr(h->red_out); fr(h->counter); fr(h->staging_dev); fr(h->nn_id); fr(h->nn_d2);
   fr(h->lm_partL); fr(h->lm_partE); fr(h->lm_barrier);
   voxelmap_free(h->vox);
-  if (h->h_lm) cudaFreeHost(h->h_lm);
+  h->lm.free();
   if (h->h_red) cudaFreeHost(h->h_red);
-  if (h->h_map) cudaFreeHost(h->h_map);
+  h->map.free();
   if (h->h_stage) cudaFreeHost(h->h_stage);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
@@ -1813,7 +1759,7 @@ int gsicp_gicp_align(gsicp_gicp* h, const float guess[16], float out[16]) {
   // VGICP always runs the host-driven loop.
   if (!h->vgicp && !h->host_lm && !h->timing && (h->shard_count <= 1 || h->comm) && (le - lb) <= kLmPersistentMax) {
     // device-resident LM loop: one persistent kernel, zero host round trips inside the loop
-    if (h->d_lm) std::memset(h->h_lm->H, 0, sizeof(h->h_lm->H));
+    if (h->lm.h) std::memset(h->lm.h->H, 0, sizeof(h->lm.h->H));
     iters = run_align_device(h, x0);
     if (iters < 0) return iters;
   } else {

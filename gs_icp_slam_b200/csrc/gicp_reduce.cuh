@@ -4,6 +4,7 @@
 #pragma once
 #include "gicp_math.cuh"
 #include "comm.cuh"
+#include "host_common.h"
 
 namespace gsicp {
 
@@ -80,10 +81,7 @@ __device__ __forceinline__ void block_reduce_finalize(double* v, double* __restr
     }
     if (threadIdx.x == 0) {
       *counter = 0u;  // ready for the next launch
-      if (host_seq) {
-        *host_seq = seq;
-        __threadfence_system();
-      }
+      if (host_seq) publish_seq(host_seq, seq);
     }
   }
 }

@@ -1,10 +1,12 @@
-// host_common.h — host-side helpers shared by every translation unit of libgsicp_b200.so.
+// host_common.h — host-side helpers shared by every translation unit of libgsicp_b200.so (and the device half of the
+// mailbox protocol).
 #pragma once
 #include <cuda_runtime.h>
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdint>
+#include <cstring>
 #include "../../include/gsicp_b200.h"
 
 namespace gsicp {
@@ -76,5 +78,46 @@ struct Scratch {
   template <typename T>
   T* as() const { return reinterpret_cast<T*>(ptr); }
 };
+
+// ---- mailbox: values a kernel publishes to the host without a blocking copy -------------------------------------------
+// The kernel writes its payload into mapped pinned memory and then publish_seq() stores a sequence word; the host spins in
+// wait_published() until the word holds the sequence number it expects and then reads the payload.  Each caller owns its
+// payload layout and its sequence counter.
+
+// n zeroed elements of mapped pinned host memory (h) and their device alias (d).  alloc() allocates on the first call
+// only; free() releases the block.
+template <typename T>
+struct Mapped {
+  T* h = nullptr;
+  T* d = nullptr;
+  cudaError_t alloc(size_t n) {
+    if (h) return cudaSuccess;
+    cudaError_t e = cudaHostAlloc((void**)&h, n * sizeof(T), cudaHostAllocMapped);
+    if (e != cudaSuccess) {
+      h = nullptr;
+      return e;
+    }
+    std::memset((void*)h, 0, n * sizeof(T));
+    e = cudaHostGetDevicePointer((void**)&d, h, 0);
+    if (e != cudaSuccess) free();
+    return e;
+  }
+  void free() {
+    if (h) cudaFreeHost(h);
+    h = d = nullptr;
+  }
+};
+
+// Spin until *word == seq.  Every 2^20 spins the stream is queried, so that a failed kernel ("<what> failed: ...") or a
+// stream that went idle without publishing ("<what> was not published") returns GSICP_ECUDA instead of hanging.
+int wait_published(const volatile unsigned long long* word, unsigned long long seq, cudaStream_t stream, const char* what);
+
+#ifdef __CUDACC__
+// Device half: call after the payload stores.  The fence makes the payload visible to the host before the sequence word.
+__device__ __forceinline__ void publish_seq(volatile unsigned long long* word, unsigned long long seq) {
+  __threadfence_system();
+  *word = seq;
+}
+#endif
 
 }  // namespace gsicp

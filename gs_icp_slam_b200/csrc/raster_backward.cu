@@ -18,13 +18,12 @@
 //
 // per-Gaussian backward: computeCov2D backward and the preprocess backward are one kernel (the
 // intermediate dL_dcov3D / dL_dmeans never round-trip through HBM between two launches).
-#include <cub/cub.cuh>
 #include <algorithm>
 #include <cstdlib>
 #include <mutex>
 #include <random>
 #include <vector>
-#include "host_common.h"
+#include "flag_count.cuh"
 #include "raster_common.cuh"
 #include "comm.cuh"
 
@@ -927,14 +926,6 @@ struct VisibleFlag {
   __host__ __device__ uint32_t operator()(int i) const { return radii[i] > 0 ? 1u : 0u; }
 };
 
-__global__ void publish_visible_kernel(int P, const uint32_t* __restrict__ excl, const int32_t* __restrict__ radii,
-                                       volatile unsigned long long* host_map, unsigned long long seq) {
-  host_map[0] = (unsigned long long)(excl[P - 1] + (radii[P - 1] > 0 ? 1u : 0u));
-  __threadfence_system();
-  host_map[1] = seq;
-  __threadfence_system();
-}
-
 template <bool kGather>
 __global__ void moments_compact_kernel(int P, const int32_t* __restrict__ radii, const uint32_t* __restrict__ excl,
                                        float* __restrict__ moments, float* __restrict__ dense) {
@@ -1035,46 +1026,21 @@ struct BwdShared {
   gsicp_allreduce_f32_fn fn = nullptr;
   void* user = nullptr;
   Scratch excl, dense, cub_tmp;
-  unsigned long long* h_map = nullptr;
-  unsigned long long* d_map = nullptr;
+  Mapped<unsigned long long> map;  // [0] visible Gaussians, [1] sequence word
   unsigned long long seq = 0;
 };
 static BwdShared g_bwd;
 
 static int allreduce_visible_moments(int P, const int32_t* d_radii, float* moments, cudaStream_t stream) {
   std::lock_guard<std::mutex> lock(g_bwd.mu);
-  if (!g_bwd.h_map) {
-    GSICP_CUDA(cudaHostAlloc((void**)&g_bwd.h_map, 2 * sizeof(unsigned long long), cudaHostAllocMapped));
-    g_bwd.h_map[0] = g_bwd.h_map[1] = 0;
-    GSICP_CUDA(cudaHostGetDevicePointer((void**)&g_bwd.d_map, g_bwd.h_map, 0));
-  }
-  if (int e = g_bwd.excl.ensure((size_t)P * 4)) return e;
-  cub::CountingInputIterator<int> counting(0);
-  cub::TransformInputIterator<uint32_t, VisibleFlag, cub::CountingInputIterator<int>> flags(counting, VisibleFlag{d_radii});
-  size_t tmp = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tmp, flags, g_bwd.excl.as<uint32_t>(), P, stream);
-  if (int e = g_bwd.cub_tmp.ensure(tmp)) return e;
-  tmp = g_bwd.cub_tmp.cap;
-  GSICP_CUDA(cub::DeviceScan::ExclusiveSum(g_bwd.cub_tmp.ptr, tmp, flags, g_bwd.excl.as<uint32_t>(), P, stream));
+  GSICP_CUDA(g_bwd.map.alloc(2));
+  if (int e = flag_scan<uint32_t>(P, VisibleFlag{d_radii}, g_bwd.excl, g_bwd.cub_tmp, stream)) return e;
   const unsigned long long seq = ++g_bwd.seq;
-  GSICP_LAUNCH(publish_visible_kernel, 1, 1, 0, stream, P, g_bwd.excl.as<uint32_t>(), d_radii,
-               (volatile unsigned long long*)g_bwd.d_map, seq);
+  GSICP_LAUNCH(publish_flag_count_kernel, 1, 1, 0, stream, P, g_bwd.excl.as<uint32_t>(), VisibleFlag{d_radii}, &g_bwd.map.d[0],
+               &g_bwd.map.d[1], seq);
   GSICP_CUDA(cudaGetLastError());
-  volatile unsigned long long* pm = g_bwd.h_map;
-  long spins = 0;
-  while (pm[1] != seq) {
-#if defined(__x86_64__)
-    __builtin_ia32_pause();
-#endif
-    if ((++spins & 0xfffff) == 0) {
-      const cudaError_t q = cudaStreamQuery(stream);
-      if (q != cudaSuccess && q != cudaErrorNotReady) {
-        set_error("rasterizer backward failed: %s", cudaGetErrorString(q));
-        return GSICP_ECUDA;
-      }
-    }
-  }
-  const size_t V = (size_t)pm[0];
+  if (int e = wait_published(&g_bwd.map.h[1], seq, stream, "visible count")) return e;
+  const size_t V = (size_t)g_bwd.map.h[0];
   if (V == 0) return GSICP_OK;
   if (int e = g_bwd.dense.ensure(V * kG * sizeof(float))) return e;
   GSICP_LAUNCH(moments_compact_kernel<true>, (P + 255) / 256, 256, 0, stream, P, d_radii, g_bwd.excl.as<uint32_t>(), moments,

@@ -249,9 +249,7 @@ tile_scan_kernel(int tiles, const uint32_t* __restrict__ tile_count, uint2* __re
     host_map[0] = (unsigned long long)s_warp[31];  // R
     host_map[2] = (unsigned long long)s_max[0];    // largest tile
     host_map[3] = (unsigned long long)n_big;       // tiles with >= kBigTileBin^2 instances (they lead `order`)
-    __threadfence_system();
-    host_map[1] = seq;
-    __threadfence_system();
+    publish_seq(&host_map[1], seq);
   }
   __syncthreads();
   for (int t = t0; t < t1; t++) order[atomicAdd(&s_start[min(63, (int)sqrtf((float)tile_count[t]))], 1u)] = (uint32_t)t;
@@ -461,8 +459,8 @@ constexpr int kMaxDevices = 32;
 struct FwdScratch {
   std::mutex mu;
   Scratch per_gaussian, per_instance, cub_tmp;
-  unsigned long long* h_map = nullptr;  // mapped pinned: [0] = num_rendered, [1] = sequence word, [2] = largest tile
-  unsigned long long* d_map = nullptr;
+  // [0] = num_rendered, [1] = sequence word, [2] = largest tile, [3] = tiles of the big sort class
+  Mapped<unsigned long long> map;
   unsigned long long seq = 0;
   bool sort_attr_set = false;  // cudaFuncSetAttribute of the big tile sort, per device
 };
@@ -521,11 +519,7 @@ extern "C" int gsicp_raster_forward(const gsicp_raster_args* args, float* d_out_
   }
   FwdScratch& g_fwd = g_fwd_dev[dev];
   std::lock_guard<std::mutex> lock(g_fwd.mu);
-  if (!g_fwd.h_map) {
-    GSICP_CUDA(cudaHostAlloc((void**)&g_fwd.h_map, 4 * sizeof(unsigned long long), cudaHostAllocMapped));
-    g_fwd.h_map[0] = g_fwd.h_map[1] = g_fwd.h_map[2] = 0;
-    GSICP_CUDA(cudaHostGetDevicePointer((void**)&g_fwd.d_map, g_fwd.h_map, 0));
-  }
+  GSICP_CUDA(g_fwd.map.alloc(4));
 
   int R = 0;
   unsigned long long max_tile = 0;
@@ -570,36 +564,18 @@ extern "C" int gsicp_raster_forward(const gsicp_raster_args* args, float* d_out_
     {
       ProfScope ps(kProfDepthSort, stream);  // slot reused: "tile_scan"
       GSICP_LAUNCH(tile_scan_kernel, 1, 1024, 0, stream, tiles, tile_count, img.ranges, cursor, seg_begin, seg_end,
-                   img.tile_order, (volatile unsigned long long*)g_fwd.d_map, seq);
+                   img.tile_order, g_fwd.map.d, seq);
     }
     GSICP_CUDA(cudaGetLastError());
-    {
-      volatile unsigned long long* pm = g_fwd.h_map;
-      long spins = 0;
-      while (pm[1] != seq) {
-#if defined(__x86_64__)
-        __builtin_ia32_pause();
-#endif
-        if ((++spins & 0xfffff) == 0) {
-          const cudaError_t q = cudaStreamQuery(stream);
-          if (q != cudaSuccess && q != cudaErrorNotReady) {
-            set_error("rasterizer forward failed before binning: %s", cudaGetErrorString(q));
-            return GSICP_ECUDA;
-          }
-          if (q == cudaSuccess && pm[1] != seq) {
-            set_error("instance count was not published");
-            return GSICP_ECUDA;
-          }
-        }
-      }
-      if (pm[0] > 0x7fffffffull) {
-        set_error("gsicp_raster_forward: instance count overflow");
-        return GSICP_EINVAL;
-      }
-      R = (int)pm[0];
-      max_tile = pm[2];
-      n_big = (int)pm[3];
+    const unsigned long long* pm = g_fwd.map.h;
+    if (int e = wait_published(&pm[1], seq, stream, "instance count")) return e;
+    if (pm[0] > 0x7fffffffull) {
+      set_error("gsicp_raster_forward: instance count overflow");
+      return GSICP_EINVAL;
     }
+    R = (int)pm[0];
+    max_tile = pm[2];
+    n_big = (int)pm[3];
   } else {
     GSICP_CUDA(cudaMemsetAsync(img.ranges, 0, sizeof(uint2) * tiles, stream));
   }
